@@ -5,9 +5,11 @@
     python bench.py --impl reference --gpus N ...             # the reference's own code on the host cores (oracle/_ref)
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
-Workload (config.workload): BASELINE.json configs[1] at N=1 — LLaMA-3-8B + SigLIP-SO400M-14@384, bf16
-instruction-tune step (forward + backward + AdamW), seq_len 4096, batch 4 per GPU, 4 images per sample
-(2 prompt-side, 2 answer-side), synthetic seeded data, random-init weights. N>1: the same per-GPU batch
+Workload (config.workload): LLaMA-3-8B widths (8 of its 32 decoder layers, 2.8 B trainable parameters) + SigLIP-SO400M-14@384,
+bf16 instruction-tune step (forward + backward + AdamW), seq_len 4096, batch 4 per GPU, 4 images per sample
+(2 prompt-side, 2 answer-side), synthetic seeded data, random-init weights. Depth 8 keeps the weights, the fp32
+AdamW state (14 bytes per trainable parameter) and the activations of one step inside an 80 GB H100; all 32
+layers would need about 112 GB for the optimizer alone. N>1: the same per-GPU batch
 on every rank (weak scaling, configs[2] shape at N=8 with --batch 8), one gradient all-reduce per bucket.
 Metric: interleaved tokens/sec of the whole job (sum over ranks of B*T per step / max-over-ranks time).
 """
@@ -35,9 +37,12 @@ def parse():
     ap.add_argument("--batch", type=int, default=4, help="samples per GPU")
     ap.add_argument("--seq-len", type=int, default=4096)
     ap.add_argument("--images-per-sample", type=int, default=4, help="half prompt-side, half answer-side")
-    ap.add_argument("--layers", type=int, default=32, help="debug only: fewer layers => invalid as a result")
+    ap.add_argument("--layers", type=int, default=8, help="LLaMA decoder layers (32 = the full 8B model, needs > 80 GB)")
     ap.add_argument("--save-gu-layers", type=int, default=int(os.environ.get("MM_SAVE_GU_LAYERS", "32")))
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="after the timed steps, write the last step's losses and a fixed sample of the updated weights "
+                         "as DIR/<name>.npy")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-decode", action="store_true")
     ap.add_argument("--no-shard", action="store_true", help="A/B only: replicate the optimizer state (round-1 behaviour)")
@@ -59,7 +64,7 @@ def train_flops_per_step(B, T, n_images, L=32, H=4096, I=14336, V=128258, Hq=32,
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, gpu_index):
         self.rows, self.proc, self.gpu = [], None, gpu_index
@@ -212,7 +217,7 @@ def cpu_decode_baseline():
                       f"({full / summ['executed_flops']:.2f}x). The reference decodes one sequence at a time."}
 
 
-def decode_bench(model, dev, peaks, batch=8, prompt_len=128, new_positions=512):
+def decode_bench(model, dev, peaks, layers, batch=8, prompt_len=128, new_positions=512):
     """BASELINE.json configs[3]: 512-position greedy decode, batch 8, KV cache, mixed text + 4 x 64 visual-token
     embeddings per sequence. Weights are random, so emission follows a forced schedule (SURVEY.md section 8d);
     every step still runs lm_head + argmax + the vision head / projector feedback."""
@@ -244,10 +249,10 @@ def decode_bench(model, dev, peaks, batch=8, prompt_len=128, new_positions=512):
     n_vis = sum(int(x.shape[0]) for x in imgs)
     n_txt = sum(int(x.numel()) for x in ids)
     steps = new_positions
-    P = 7504666624
-    kv_bytes = sum(2 * 8 * 128 * 2 * 32 * (prompt_len + t) for t in range(steps)) * batch
+    P = layers * 218103808 + 4096 * 128256                 # decoder + lm_head weights read per step
+    kv_bytes = sum(2 * 8 * 128 * 2 * layers * (prompt_len + t) for t in range(steps)) * batch
     bytes_total = steps * (P * 2 + (4096 * 4096 + 4096 * 1152 + 1152 * 4096 + 4096 * 4096) * 2) + kv_bytes
-    hbm = peaks.get("hbm_gbs", 6650.0)
+    hbm = peaks.get("hbm_gbs", 3350.0)
     achieved = bytes_total / (ms / 1e3) / 1e9
     model.train()
     return {"metric": f"decode tokens/sec (512 new positions incl. 256 visual embeddings, batch {batch}, KV cache)",
@@ -306,7 +311,7 @@ def preprocess_bench(dev, peaks, n_images=16, h=480, w=640, iters=20):
             op.siglip_preprocess(im)
         cpu = {"value": 4 / (time.perf_counter() - t0), "unit": "images/s", "cores": 1, "kind": "port",
                "sample": "4 images through oracle/preprocess.py (numpy)"}
-    hbm = peaks.get("hbm_gbs", 6650.0)
+    hbm = peaks.get("hbm_gbs", 3350.0)
     return {"metric": "SigLIP image pre-processing, host uint8 -> device fp32 [N,3,384,384]", "bit_exact_vs_oracle": ok,
             "value": n_images / wall, "unit": "images/s", "device_ms_per_batch": dev_ms, "wall_ms_per_batch": wall * 1e3,
             "images_per_batch": n_images, "input": f"{w}x{h} RGB uint8", "h2d_bytes_per_batch": in_bytes,
@@ -355,6 +360,27 @@ def run_reference_impl(args):
             "gpu_launches": 0}
     print(json.dumps(line), flush=True)
     return 0
+
+
+def dump_outputs(out_dir, out, model, layers, sample=65536):
+    """What the timed path hands its caller after the last timed step: the three losses (float64) and, because the
+    step updates the weights in place, a fixed sample of the updated trainable parameters (float32; the indices
+    depend only on the parameter's size, so two builds can be compared output for output)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    for k in ("loss", "loss_language", "loss_image_ar"):
+        np.save(os.path.join(out_dir, f"{k}.npy"), out[k].detach().double().reshape(-1).cpu().numpy())
+    keep = ("model.layers.0.", f"model.layers.{layers - 1}.", "lm_head.", "model.embed_tokens.", "model.norm.",
+            "mm_projector.", "vision_head.")
+    for name, p in model.named_parameters():
+        if not p.requires_grad or not any(k in name for k in keep):
+            continue
+        flat = p.detach().reshape(-1)
+        if flat.numel() > sample:
+            idx = torch.randint(0, flat.numel(), (sample,), generator=torch.Generator().manual_seed(flat.numel()))
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(out_dir, f"{name}.npy"), flat.float().cpu().numpy())
 
 
 # ------------------------------------------------------------------------------------------------
@@ -425,7 +451,7 @@ def main():
             ops.GEMM_PROFILE = []
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        last = None
+        last = out = None
         for _ in range(steps):
             out = engine.step(batch)
             if read_loss:
@@ -442,19 +468,21 @@ def main():
             t = torch.tensor([ms], device=dev)
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
             ms = float(t)
-        return ms, launches, prof, float(last)
+        return ms, launches, prof, float(last), out
 
     for _ in range(args.warmup):
         engine.step(dev_batch)
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
-    ms, launches, prof, loss_val = timed(dev_batch, args.steps, read_loss=False, profile_gemm=True)
+    ms, launches, prof, loss_val, last_out = timed(dev_batch, args.steps, read_loss=False, profile_gemm=True)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_out, model, args.layers)
     tokens_per_step = world * B * T
     value = tokens_per_step * args.steps / (ms / 1e3)
 
-    # roofline of the dominant kernel family (tcgen05 GEMM): algorithmic flops / measured launch time
+    # roofline of the dominant kernel family (wgmma GEMM): algorithmic flops / measured launch time
     gemm_ms = sum(a.elapsed_time(b) for a, b, _ in prof)
     gemm_flops = sum(f for _, _, f in prof)
     peaks = {}
@@ -466,18 +494,12 @@ def main():
     peak = peaks.get("bf16_tflops_sustained")
     peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)"
     if peak is None:
-        peak, peak_src = 1400.0, "fallback (B200_PROFILING.md sustained)"
+        peak, peak_src = 989.0, "NVIDIA H100 SXM data sheet, dense BF16 at 700 W (not a measured rate)"
     achieved = gemm_flops / (gemm_ms / 1e3) / 1e12 if gemm_ms > 0 else 0.0
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02_gemm_ncu_summary.json")) as f:
-            traffic = json.load(f).get("dram_bytes_per_launch")
-    except Exception:  # noqa: BLE001
-        pass
     step_flops = train_flops_per_step(B, T, n_images, L=args.layers)
-    roofline = {"bound": "tensor", "kernel": "gemm_tcgen05_kernel (all dense contractions of the step)",
+    roofline = {"bound": "tensor", "kernel": "gemm_wgmma_kernel (all dense contractions of the step)",
                 "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                "traffic": traffic, "peak_source": peak_src, "launches": len(prof),
+                "peak_source": peak_src, "launches": len(prof),
                 "gemm_share_of_step": gemm_ms / ms if ms > 0 else None,
                 "step_algorithmic_tflop": step_flops / 1e12,
                 "step_achieved_tflops_per_gpu": step_flops * args.steps / (ms / 1e3) / 1e12,
@@ -485,7 +507,7 @@ def main():
 
     e2e = None
     if not args.no_e2e:
-        ms2, _, _, _ = timed(host_batch, args.steps, read_loss=True)
+        ms2, _, _, _, _ = timed(host_batch, args.steps, read_loss=True)
         h2d = host_batch["images"].numel() * 2 + (host_batch["input_ids"].numel() * 4 * 3)
         e2e = {"value": tokens_per_step * args.steps / (ms2 / 1e3), "unit": UNIT, "ms_per_step": ms2 / args.steps,
                "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": 4,
@@ -521,7 +543,7 @@ def main():
                 db["images"] = hb["images"].to(dev)
                 for _ in range(2):
                     engine.step(db)
-                ms_x, _, _, loss_x = timed(db, 3, read_loss=False)
+                ms_x, _, _, loss_x, _ = timed(db, 3, read_loss=False)
                 fl = train_flops_per_step(b_x, t_x, b_x * imgs_x, L=args.layers)
                 extra[key] = {"value": world * b_x * t_x * 3 / (ms_x / 1e3), "unit": UNIT, "ms_per_step": ms_x / 3,
                               "batch_per_gpu": b_x, "global_batch": world * b_x, "seq_len": t_x, "images_per_sample": imgs_x,
@@ -544,14 +566,14 @@ def main():
     decode = None
     if rank == 0 and world == 1 and not args.no_decode:
         try:
-            decode = decode_bench(model, dev, peaks)
+            decode = decode_bench(model, dev, peaks, args.layers)
             decode["cpu_baseline"] = cpu_decode
         except Exception as e:  # noqa: BLE001 - secondary metric must not lose the headline line
             decode = {"error": repr(e)[:300]}
         if "error" not in decode:
             # beyond BASELINE's batch 8: 32 sequences share every weight byte of the step (four n8 tiles of the same MMAs)
             try:
-                d32 = decode_bench(model, dev, peaks, batch=32)
+                d32 = decode_bench(model, dev, peaks, args.layers, batch=32)
                 decode["batch32"] = {k: d32[k] for k in ("metric", "value", "unit", "ms_per_step", "roofline")}
             except Exception as e:  # noqa: BLE001 - an extra key must not lose the batch-8 decode line
                 decode["batch32"] = {"error": repr(e)[:300]}
@@ -567,7 +589,7 @@ def main():
                                        f"(fwd+bwd+AdamW fp32 master), seq_len {T}, batch {B}/GPU, {n_images // B} images/sample "
                                        "(64 visual tokens each), synthetic seeded inputs, random-init weights",
                            "global_batch": world * B, "seq_len": T, "parallelism": f"dp{world}",
-                           "l2_policy": "inputs+weights (>100 GB/step) far exceed the 126 MB L2; no flush needed",
+                           "l2_policy": "inputs+weights (tens of GB per step) far exceed the 50 MB L2; no flush needed",
                            "max_grad_norm": None,
                            "optimizer": "AdamW fused into the backward sweep, fp32 master/m/v " +
                                         ((f"sharded over the {world} ranks (ZeRO-1: " + ("" if getattr(engine, "fused_reduce", False) else "NCCL reduce-scatter -> ") + "AdamW on the slice, "

@@ -1,4 +1,4 @@
-/* metamorph_b200 — C ABI of the B200 (sm_100a) hot-path kernels.
+/* metamorph_b200 — C ABI of the H100 (sm_90a) hot-path kernels.
  *
  * The reference (facebookresearch/metamorph) has NO native/FFI layer: its hot path is Python calling
  * third-party torch / transformers ops (SURVEY.md F1, F3). This header is therefore the boundary the
@@ -10,6 +10,9 @@
  *     mm_last_error() returns a thread-local message. No exceptions cross the ABI.
  *   - the caller owns every buffer (including workspaces); kernels never allocate or free.
  *   - all work is enqueued asynchronously on the given cudaStream_t; device pointers only.
+ *   - mm_ce_fwd_bwd / mm_cosine_loss (with loss_sum) and mm_rmsnorm_bwd (with dw_accum) use library-owned device
+ *     scratch private to (device, stream), allocated on a stream's first such call: calls on one stream share it in
+ *     stream order, calls on different streams never do. The first call on a stream must not be inside graph capture.
  *   - matrices are row-major bf16 unless stated; `ld*` are row pitches in elements.
  */
 #ifndef METAMORPH_B200_H
@@ -21,9 +24,9 @@ extern "C" {
 
 const char* mm_last_error(void);
 int mm_abi_version(void);
-int mm_check_device(void); /* 0 iff the current device is sm_100 */
+int mm_check_device(void); /* 0 iff the current device is sm_90 (H100) */
 
-/* Dense contraction on tcgen05 tensor cores (TMA -> 128B-swizzled smem -> tcgen05.mma -> TMEM -> epilogue).
+/* Dense contraction on Hopper tensor cores (TMA -> 128B-swizzled smem -> wgmma.mma_async -> registers -> epilogue).
  * Replaces every nn.Linear / F.linear on the path: HF LlamaAttention q/k/v/o_proj (modeling_llama.py:262-288),
  * LlamaMLP (:182-183), lm_head (metamorph_llama.py:398), mm_projector (metamorph_arch.py:159), vision_head
  * (metamorph_llama.py:433), SigLIP projections / MLP / patch-embed (modeling_siglip.py:178-184,285-326) and,
@@ -111,7 +114,7 @@ int mm_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse
                 long long ldq, long long ldk, long long ldv, long long ldo, int B, int T, int Hq, int Hkv,
                 int head_dim, int causal, float scale, cudaStream_t s);
 long long mm_attn_bwd_workspace_bytes(int B, int T, int Hq);
-/* tcgen05 / TMEM / TMA flash attention for head_dim 128 (csrc/attention_tc.cu forward, csrc/attention_bwd_tc.cu backward:
+/* wgmma / TMA flash attention for head_dim 128 (csrc/attention_tc.cu forward, csrc/attention_bwd_tc.cu backward:
  * a query-stationary dQ kernel + a key-stationary dK/dV kernel, no atomics -> bit-reproducible); same contracts as above.
  * Rows >= seqlens[b] are outside the sequence: zero dQ/dK/dV, their dO is ignored. Backward workspace: lse*log2e and
  * delta, mm_attn_bwd_tc_workspace_bytes. */

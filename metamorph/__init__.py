@@ -1,3 +1,3 @@
-"""Drop-in alias package: `import metamorph.model`, `metamorph.train.train`, ... resolve to the B200
+"""Drop-in alias package: `import metamorph.model`, `metamorph.train.train`, ... resolve to the H100
 implementation (metamorph_b200). Lets reference call sites switch without editing imports."""
 from metamorph_b200.model import MetaMorphLlamaForCausalLM  # noqa: F401

@@ -1,4 +1,4 @@
-"""metamorph_b200 — B200-native (sm_100a) implementation of MetaMorph's data-parallel hot path.
+"""metamorph_b200 — H100-native (sm_90a) implementation of MetaMorph's data-parallel hot path.
 
 Public surface mirrors the reference package (`metamorph.model.MetaMorphLlamaForCausalLM`,
 `metamorph.train.train.train`, `inference.load_metamorph.load_metamorph_model`); see DESIGN.md.

@@ -1,4 +1,4 @@
-"""In-tree build of the sm_100a CUDA extension (`metamorph_b200/_C.so`).
+"""In-tree build of the sm_90a CUDA extension (`metamorph_b200/_C.so`).
 
 nvcc cross-compiles without a GPU; the resulting shared library exports a plain C ABI
 (see include/metamorph_b200.h) and is loaded with ctypes by `metamorph_b200._lib`.
@@ -17,8 +17,9 @@ CSRC = PKG / "csrc"
 BUILD = PKG.parent / "build" / "obj"
 SO = PKG / "_C.so"
 
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]   # H100 (Hopper): wgmma / setmaxnreg need the "a" target
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *ARCH,
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
     "--expt-relaxed-constexpr",
@@ -60,7 +61,7 @@ def _compile_one(src: Path, verbose: bool) -> Path:
 
 
 def build(verbose: bool = True, force: bool = False) -> Path:
-    """Compile every csrc/*.cu for sm_100a and link metamorph_b200/_C.so."""
+    """Compile every csrc/*.cu for sm_90a and link metamorph_b200/_C.so."""
     BUILD.mkdir(parents=True, exist_ok=True)
     srcs = sorted(CSRC.glob("*.cu"))
     if force:
@@ -72,7 +73,7 @@ def build(verbose: bool = True, force: bool = False) -> Path:
     sig = " ".join(o.name for o in objs)
     if SO.exists() and stamp.exists() and stamp.read_text() == sig and not force:
         return SO
-    cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(SO),
+    cmd = [_nvcc(), "-shared", *ARCH, "-o", str(SO),
            *map(str, objs), "-cudart", "static"]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:

@@ -76,7 +76,7 @@ def require_cuda(*tensors) -> None:
     for t in tensors:
         if t is not None and not t.is_cuda:
             raise MetaMorphB200Error(
-                "metamorph_b200 kernels run on CUDA (sm_100a) tensors only; got a CPU tensor. "
+                "metamorph_b200 kernels run on CUDA (sm_90a) tensors only; got a CPU tensor. "
                 "There is no CPU fallback on the product path.")
 
 

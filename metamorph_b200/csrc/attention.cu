@@ -3,8 +3,8 @@
 // registers (exp2 domain, warp-shuffle row reductions), O(T) memory.
 //
 // Round-1 implementation uses the legacy warp-level tensor path (ldmatrix + mma.sync m16n8k16,
-// SASS HMMA) with cp.async double-buffered K/V tiles; the tcgen05/TMEM rewrite of this file is the
-// next optimisation step (DESIGN.md "what comes next").  The backward accumulates dQ with the TMA
+// SASS HMMA) with cp.async double-buffered K/V tiles; the product path runs the wgmma kernels of
+// attention_tc.cu / attention_bwd_tc.cu; these stay as the tests' comparison kernels.  The backward accumulates dQ with the TMA
 // engine's bulk reduce-add (cp.reduce.async.bulk ... .add.f32, smem -> global fp32) instead of
 // per-lane atomics, and keeps dK/dV in registers across the query heads of a GQA group.
 //
@@ -556,7 +556,7 @@ int launch_fwd(const FwdParams& p, cudaStream_t stream) {
 
 }  // namespace
 
-// Shared by the mma.sync and tcgen05 backward paths (declared in common.cuh).
+// Shared by the mma.sync and wgmma backward paths (declared in common.cuh).
 MM_API int mm_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse,
                        const int* seqlens, long long ldq, long long ldk, long long ldv,
                        long long ldo, int B, int T, int Hq, int Hkv, int head_dim, int causal,

@@ -1,29 +1,18 @@
-// metamorph_b200 — flash attention BACKWARD on tcgen05 (head_dim 128, causal, GQA): two software-pipelined kernels.
-// (Backward of SURVEY.md K12: HF modeling_llama.py:199-220 / SDPA under autograd; reference call site
-// metamorph_llama.py:349-359 via loss.backward().)
+// metamorph_b200 — flash attention BACKWARD on Hopper tensor cores (wgmma + TMA + mbarrier; head_dim 128, causal,
+// GQA): two kernels. (Backward of SURVEY.md K12: HF modeling_llama.py:199-220 / SDPA under autograd; reference call
+// site metamorph_llama.py:349-359 via loss.backward().)
 //
-//   kernel 1  flash_bwd_dq_kernel   query-stationary: one CTA = 128 queries of one (batch, q-head). Lanes = queries.
+//   kernel 1  flash_bwd_dq_kernel   query-stationary: one CTA = 128 queries of one (batch, q-head); two consumer
+//             warpgroups own 64 queries each. Per 128-key tile, in two halves of 64 keys:
 //             delta = rowsum(dO o O) (preamble, from the TMA tiles)   -> also written for kernel 2, with lse*log2(e)
-//             S  = Q  K_j^T   (SS)          -> TMEM, double-buffered
-//             dP = dO V_j^T   (SS)          -> TMEM
-//             dS = P o (dP - delta) * scale    elementwise, packed bf16 INSIDE each warp's own dP columns
-//             dQ += dS K_j    (TS: A = dS in TMEM, B = K_j MN-major from the same TMA tile) -> TMEM, stored once as bf16
+//             S  = Q  K^T,  dP = dO V^T      (wgmma, operands K-major in shared memory, results in registers)
+//             dS = P o (dP - delta) * scale   elementwise on the accumulator fragments, packed to bf16 A fragments
+//             dQ += dS K                      (A = dS from registers, B = K MN-major from the same TMA tile)
 //   kernel 2  flash_bwd_dkv_kernel  key-stationary: one CTA = 128 keys of one (batch, kv-head); loops over the G query
-//             heads of the group and the query tiles at/after the key tile, in the TRANSPOSED orientation (lanes = keys):
-//             S^T  = K Q^T,  dP^T = V dO^T  (SS);  P^T, dS^T elementwise (no row reductions: lse / delta per column);
-//             dV += P^T dO,  dK += dS^T Q   (TS, B = dO / Q MN-major); dK, dV stay in TMEM for the whole CTA.
-//
-// Round 1 computed dQ inside the key-stationary kernel: a third product per tile through a swizzled smem copy of dS^T
-// (18.6 M bank conflicts per launch), 4.4 GB of red.global.add.f32 per launch into a zeroed fp32 buffer, a memset and a
-// convert kernel, with the MMA and elementwise phases serialised (454 TFLOP/s). Here every product reads its dS / P
-// operand from TMEM, nothing is reduced through global memory (the backward is bit-reproducible), and both kernels
-// overlap the elementwise phase of one tile with the MMAs of its neighbours:
-//   * each elementwise warp packs its bf16 results into the first half of ITS OWN 32 fp32 columns (the k-step of a
-//     TS-form MMA can point at any TMEM column, so the A operand need not be contiguous) -> no cross-warp hazard and no
-//     block-wide barrier between the TMEM loads and stores of a tile;
-//   * the elementwise work is split in two phases (P from S, then dS from dP) with their own mbarriers, so the tensor
-//     core runs {dV_i, S_{i+1}} under phase 2 of tile i and {dK_i, dP_{i+1}} under phase 1 of tile i+1.
-// Cost: S and dP are computed twice (7 products per tile pair instead of 5).
+//             heads of the group and the query tiles at/after the key tile, in the TRANSPOSED orientation:
+//             S^T = K Q^T,  dP^T = V dO^T;  P^T, dS^T elementwise (lse / delta per column, from shared memory);
+//             dV += P^T dO,  dK += dS^T Q   (B = dO / Q MN-major); dK, dV stay in registers for the whole CTA.
+// Nothing is reduced through global memory, so the backward is bit-reproducible.
 //
 // Rows beyond a sample's length (seqlens[b] <= row < T, right padding) are not part of the sequence: they receive zero
 // dQ/dK/dV and contribute nothing, exactly as the reference's masked positions carry no gradient (their q/k/v/dO values
@@ -34,7 +23,7 @@ using namespace mm_attn_tc;
 
 namespace {
 
-constexpr int BW_THREADS = 576;  // TMA warp + MMA warp + 16 elementwise warps
+constexpr int BW_THREADS = 384;  // producer warpgroup + 2 consumer warpgroups
 constexpr int BW_TILE = 32768;   // 128 x 128 bf16
 constexpr int BW_SMEM = 6 * BW_TILE + 2048 /*stats / reduction scratch*/ + 256 /*barriers*/ + 1024 /*alignment*/;
 
@@ -54,24 +43,15 @@ struct BwdTcParams {
   float scale;
 };
 
-__device__ __forceinline__ void store_bf16x32(bf16* dst, const uint32_t (&a)[32]) {
+// rows g and g + 8 of a 64 x 128 fp32 accumulator fragment -> bf16 (zero when !ok), 16 x bf16x2 stores per row
+__device__ __forceinline__ void store_acc_rows(bf16* dst0, bf16* dst1, bool w0, bool w1, bool ok0, bool ok1,
+                                               const float (&a)[64], int q2) {
 #pragma unroll
-  for (int t = 0; t < 32; t += 8) {
-    int4 o;
-    o.x = pack_bf16x2(__uint_as_float(a[t]), __uint_as_float(a[t + 1]));
-    o.y = pack_bf16x2(__uint_as_float(a[t + 2]), __uint_as_float(a[t + 3]));
-    o.z = pack_bf16x2(__uint_as_float(a[t + 4]), __uint_as_float(a[t + 5]));
-    o.w = pack_bf16x2(__uint_as_float(a[t + 6]), __uint_as_float(a[t + 7]));
-    *reinterpret_cast<int4*>(dst + t) = o;
+  for (int t = 0; t < 16; ++t) {
+    if (w0) *reinterpret_cast<uint32_t*>(dst0 + 8 * t + q2) = ok0 ? pack_bf16x2(a[4 * t], a[4 * t + 1]) : 0u;
+    if (w1) *reinterpret_cast<uint32_t*>(dst1 + 8 * t + q2) = ok1 ? pack_bf16x2(a[4 * t + 2], a[4 * t + 3]) : 0u;
   }
 }
-
-// TMEM column of the k-th 16-element slice of an elementwise result: warp chunk c = k/2 packs its 32 bf16 values into
-// the first 16 of its own 32 fp32 columns
-__device__ __forceinline__ uint32_t packed_col(int k) { return (uint32_t)((k >> 1) * 32 + (k & 1) * 8); }
-
-constexpr uint32_t kIdescKK = (1u << 4) | (1u << 7) | (1u << 10) | (uint32_t(128 >> 3) << 17) | (uint32_t(128 >> 4) << 24);
-constexpr uint32_t kIdescBmn = kIdescKK | (1u << 16);   // B operand MN-major
 
 // ======================================================================================================= kernel 1: dQ
 __global__ void __launch_bounds__(BW_THREADS, 1)
@@ -79,7 +59,7 @@ flash_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
                     const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do,
                     const __grid_constant__ CUtensorMap tmap_o, BwdTcParams p) {
   extern __shared__ uint8_t smem_raw[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int qt = p.work_q ? p.work_q[blockIdx.x].y : (int)gridDim.x - 1 - (int)blockIdx.x;   // heavy (late) tiles first
   const int h = blockIdx.y, b = p.work_q ? p.work_q[blockIdx.x].x : (int)blockIdx.z;
   const int hk = h / (p.Hq / p.Hkv);
@@ -109,227 +89,171 @@ flash_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   const uint32_t sQ = base, sdO = base + BW_TILE;
   const uint32_t sK[2] = {base + 2 * BW_TILE, base + 4 * BW_TILE};
   const uint32_t sV[2] = {base + 3 * BW_TILE, base + 5 * BW_TILE};
-  float* sRed = reinterpret_cast<float*>(base_ptr + 6 * BW_TILE);            // [4][128]
+  float* sRed = reinterpret_cast<float*>(base_ptr + 6 * BW_TILE);            // [2][128]
   const uint32_t bar = base + 6 * BW_TILE + 2048;
   const uint32_t q_full = bar, k_full0 = bar + 8, k_full1 = bar + 16, k_empty0 = bar + 24, k_empty1 = bar + 32,
-                 v_full0 = bar + 40, v_full1 = bar + 48, v_empty0 = bar + 56, v_empty1 = bar + 64, s_full0 = bar + 72,
-                 s_full1 = bar + 80, dp_full = bar + 88, ds_full = bar + 96, o_used = bar + 104, dq_done = bar + 112,
-                 tmem_slot = bar + 120;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(base_ptr + 6 * BW_TILE + 2048 + 120);
+                 v_full0 = bar + 40, v_full1 = bar + 48, v_empty0 = bar + 56, v_empty1 = bar + 64, o_used = bar + 72;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_q);
     prefetch_tmap(&tmap_k);
     prefetch_tmap(&tmap_v);
     prefetch_tmap(&tmap_do);
     prefetch_tmap(&tmap_o);
-    for (int i = 0; i < 12; ++i) mbar_init(bar + 8 * i, 1);   // q_full .. dp_full
-    mbar_init(ds_full, 16);
-    mbar_init(o_used, 16);
-    mbar_init(dq_done, 1);
+    mbar_init(q_full, 1);
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(k_full0 + 8 * i, 1);
+      mbar_init(v_full0 + 8 * i, 1);
+      mbar_init(k_empty0 + 8 * i, 8);   // one arrive per consumer warp
+      mbar_init(v_empty0 + 8 * i, 8);
+    }
+    mbar_init(o_used, 8);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<512>(tmem_slot);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem = *tmem_slot_ptr;
-  const uint32_t tS[2] = {tmem, tmem + 128};
-  const uint32_t tDP = tmem + 256, tDQ = tmem + 384;
 
-  if (warp == 0 && lane == 0) {
+  if (wg == 0) {
     // ---------------------------------------------------------------- TMA producer
-    mbar_arrive_expect_tx(q_full, 3 * BW_TILE);
-    tma_load_2d(sQ, &tmap_q, q_full, h * 128, tok0 + q0);
-    tma_load_2d(sQ + 16384, &tmap_q, q_full, h * 128 + 64, tok0 + q0);
-    tma_load_2d(sdO, &tmap_do, q_full, h * 128, tok0 + q0);
-    tma_load_2d(sdO + 16384, &tmap_do, q_full, h * 128 + 64, tok0 + q0);
-    tma_load_2d(sV[1], &tmap_o, q_full, h * 128, tok0 + q0);            // O parks in V stage 1 until delta is done
-    tma_load_2d(sV[1] + 16384, &tmap_o, q_full, h * 128 + 64, tok0 + q0);
-    for (int j = 0; j < n_tiles; ++j) {
-      const int bf = j & 1;
-      const uint32_t ph = (uint32_t)((j >> 1) & 1);
-      mbar_wait(bf ? k_empty1 : k_empty0, ph ^ 1);
-      mbar_arrive_expect_tx(bf ? k_full1 : k_full0, BW_TILE);
-      tma_load_2d(sK[bf], &tmap_k, bf ? k_full1 : k_full0, hk * 128, tok0 + j * 128);
-      tma_load_2d(sK[bf] + 16384, &tmap_k, bf ? k_full1 : k_full0, hk * 128 + 64, tok0 + j * 128);
-      mbar_wait(bf ? v_empty1 : v_empty0, ph ^ 1);
-      if (j == 1) mbar_wait(o_used, 0);
-      mbar_arrive_expect_tx(bf ? v_full1 : v_full0, BW_TILE);
-      tma_load_2d(sV[bf], &tmap_v, bf ? v_full1 : v_full0, hk * 128, tok0 + j * 128);
-      tma_load_2d(sV[bf] + 16384, &tmap_v, bf ? v_full1 : v_full0, hk * 128 + 64, tok0 + j * 128);
-    }
-  } else if (warp == 1 && lane == 0) {
-    // ---------------------------------------------------------------- MMA issuer
-    auto issue_s = [&](int j) {
-      const int bf = j & 1;
-      mbar_wait(bf ? k_full1 : k_full0, (uint32_t)((j >> 1) & 1));
-      tcgen05_fence_after();
-#pragma unroll
-      for (int k = 0; k < 8; ++k)
-        umma_bf16_ss(tS[bf], desc_kmajor(sQ, k), desc_kmajor(sK[bf], k), kIdescKK, k != 0 ? 1u : 0u);
-      umma_commit(bf ? s_full1 : s_full0);
-    };
-    auto issue_dp = [&](int j) {
-      const int bf = j & 1;
-      mbar_wait(bf ? v_full1 : v_full0, (uint32_t)((j >> 1) & 1));
-      tcgen05_fence_after();
-#pragma unroll
-      for (int k = 0; k < 8; ++k)
-        umma_bf16_ss(tDP, desc_kmajor(sdO, k), desc_kmajor(sV[bf], k), kIdescKK, k != 0 ? 1u : 0u);
-      umma_commit(bf ? v_empty1 : v_empty0);
-      umma_commit(dp_full);
-    };
-    mbar_wait(q_full, 0);
-    issue_s(0);
-    issue_dp(0);
-    for (int j = 0; j < n_tiles; ++j) {
-      const int bf = j & 1;
-      if (j + 1 < n_tiles) issue_s(j + 1);          // other S buffer: its last reader (elementwise j-1) finished before ds_full(j-1)
-      mbar_wait(ds_full, (uint32_t)(j & 1));        // dS_j packed into the dP columns by all 16 warps
-      tcgen05_fence_after();
-#pragma unroll
-      for (int k = 0; k < 8; ++k)
-        umma_bf16_ts(tDQ, tDP + packed_col(k), desc_mnmajor(sK[bf], k), kIdescBmn, (j | k) != 0 ? 1u : 0u);
-      umma_commit(bf ? k_empty1 : k_empty0);
-      if (j + 1 < n_tiles) issue_dp(j + 1);         // overwrites dS_j: issued after the dQ_j MMAs that read it
-    }
-    umma_commit(dq_done);
-  } else if (warp >= 2) {
-    // ---------------------------------------------------------------- elementwise: thread = query row r x 32 key columns
-    const int quad = warp & 3;
-    const int c = (warp - 2) >> 2;
-    const int r = quad * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(quad * 32) << 16;
-    const int q_idx = q0 + r;
-    const bool q_ok = q_idx < kv_len;
-    const float sl2 = p.scale * kLog2e;
-    // ---- preamble: delta = rowsum(dO o O) from the swizzled TMA tiles (two [128 x 64] boxes, 16-byte chunks XOR row%8)
-    mbar_wait(q_full, 0);
-    float part = 0.f;
-    {
-      const uint32_t off = (uint32_t)(c >> 1) * 16384u + (uint32_t)r * 128u;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const uint32_t slot = (uint32_t)((((c & 1) * 4 + i) ^ (r & 7)) << 4);
-        const int4 a = *reinterpret_cast<const int4*>(base_ptr + BW_TILE + off + slot);          // dO
-        const int4 o = *reinterpret_cast<const int4*>(base_ptr + 5 * BW_TILE + off + slot);      // O (V stage 1)
-        const uint32_t ua[4] = {(uint32_t)a.x, (uint32_t)a.y, (uint32_t)a.z, (uint32_t)a.w};
-        const uint32_t uo[4] = {(uint32_t)o.x, (uint32_t)o.y, (uint32_t)o.z, (uint32_t)o.w};
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          const float2 x = unpack_bf16x2(ua[t]);
-          const float2 y = unpack_bf16x2(uo[t]);
-          part = fmaf(x.x, y.x, fmaf(x.y, y.y, part));
-        }
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      mbar_arrive_expect_tx(q_full, 3 * BW_TILE);
+      tma_load_2d(sQ, &tmap_q, q_full, h * 128, tok0 + q0);
+      tma_load_2d(sQ + 16384, &tmap_q, q_full, h * 128 + 64, tok0 + q0);
+      tma_load_2d(sdO, &tmap_do, q_full, h * 128, tok0 + q0);
+      tma_load_2d(sdO + 16384, &tmap_do, q_full, h * 128 + 64, tok0 + q0);
+      tma_load_2d(sV[1], &tmap_o, q_full, h * 128, tok0 + q0);            // O parks in V stage 1 until delta is done
+      tma_load_2d(sV[1] + 16384, &tmap_o, q_full, h * 128 + 64, tok0 + q0);
+      for (int j = 0; j < n_tiles; ++j) {
+        const int bf = j & 1;
+        const uint32_t ph = (uint32_t)((j >> 1) & 1);
+        mbar_wait(bf ? k_empty1 : k_empty0, ph ^ 1);
+        mbar_arrive_expect_tx(bf ? k_full1 : k_full0, BW_TILE);
+        tma_load_2d(sK[bf], &tmap_k, bf ? k_full1 : k_full0, hk * 128, tok0 + j * 128);
+        tma_load_2d(sK[bf] + 16384, &tmap_k, bf ? k_full1 : k_full0, hk * 128 + 64, tok0 + j * 128);
+        mbar_wait(bf ? v_empty1 : v_empty0, ph ^ 1);
+        if (j == 1) mbar_wait(o_used, 0);
+        mbar_arrive_expect_tx(bf ? v_full1 : v_full0, BW_TILE);
+        tma_load_2d(sV[bf], &tmap_v, bf ? v_full1 : v_full0, hk * 128, tok0 + j * 128);
+        tma_load_2d(sV[bf] + 16384, &tmap_v, bf ? v_full1 : v_full0, hk * 128 + 64, tok0 + j * 128);
       }
     }
-    sRed[c * 128 + r] = part;
-    __syncwarp();
-    if (lane == 0) mbar_arrive(o_used);                      // this warp no longer reads the O tile
-    asm volatile("bar.sync 1, 512;" ::: "memory");
-    const float delta = q_ok ? (sRed[r] + sRed[128 + r] + sRed[256 + r] + sRed[384 + r]) * p.scale : 0.f;
-    const float lse2 = q_ok ? p.lse[((long long)b * p.Hq + h) * p.T + q_idx] * kLog2e : 0.f;
-    if (c == 0) {
-      p.delta[stat0 + r] = delta;
-      p.lse2[stat0 + r] = lse2;
-    }
-    for (int j = 0; j < n_tiles; ++j) {
-      const int bf = j & 1;
-      const int k0 = j * 128 + c * 32;                       // first key column of this thread
-      // ---- phase 1: P = exp2(S * scale*log2e - lse2)
-      mbar_wait(bf ? s_full1 : s_full0, (uint32_t)((j >> 1) & 1));
-      tcgen05_fence_after();
-      uint32_t s0[16], s1[16];
-      tmem_ld_32x32b_x16(tS[bf] + lane_off + c * 32, s0);
-      tmem_ld_32x32b_x16(tS[bf] + lane_off + c * 32 + 16, s1);
-      tmem_ld_wait();
-      const bool full_tile = q_ok && (j * 128 + 127 <= q0) && (j * 128 + 128 <= kv_len);   // no causal / length edge
-      if (full_tile) {
-#pragma unroll
-        for (int t = 0; t < 16; ++t) {
-          s0[t] = __float_as_uint(fast_exp2(fmaf(__uint_as_float(s0[t]), sl2, -lse2)));
-          s1[t] = __float_as_uint(fast_exp2(fmaf(__uint_as_float(s1[t]), sl2, -lse2)));
-        }
-      } else {
-#pragma unroll
-        for (int t = 0; t < 16; ++t) {
-          const bool ok0 = q_ok && (k0 + t <= q_idx) && (k0 + t < kv_len);
-          const bool ok1 = q_ok && (k0 + 16 + t <= q_idx) && (k0 + 16 + t < kv_len);
-          s0[t] = ok0 ? __float_as_uint(fast_exp2(fmaf(__uint_as_float(s0[t]), sl2, -lse2))) : 0u;
-          s1[t] = ok1 ? __float_as_uint(fast_exp2(fmaf(__uint_as_float(s1[t]), sl2, -lse2))) : 0u;
-        }
-      }
-      // ---- phase 2: dS = P o (dP*scale - delta), packed bf16 into this warp's own first 16 dP columns
-      mbar_wait(dp_full, (uint32_t)(j & 1));
-      tcgen05_fence_after();
-      uint32_t pk[16];
-      {   // two halves of 16 columns keep the live register set small (no spills at 576 threads per CTA)
-        uint32_t d[16];
-        tmem_ld_32x32b_x16(tDP + lane_off + c * 32, d);
-        tmem_ld_wait();
-#pragma unroll
-        for (int t = 0; t < 16; t += 2)
-          pk[t >> 1] = pack_bf16x2(__uint_as_float(s0[t]) * fmaf(__uint_as_float(d[t]), p.scale, -delta),
-                                   __uint_as_float(s0[t + 1]) * fmaf(__uint_as_float(d[t + 1]), p.scale, -delta));
-        tmem_ld_32x32b_x16(tDP + lane_off + c * 32 + 16, d);
-        tmem_ld_wait();
-#pragma unroll
-        for (int t = 0; t < 16; t += 2)
-          pk[8 + (t >> 1)] = pack_bf16x2(__uint_as_float(s1[t]) * fmaf(__uint_as_float(d[t]), p.scale, -delta),
-                                         __uint_as_float(s1[t + 1]) * fmaf(__uint_as_float(d[t + 1]), p.scale, -delta));
-      }
-      tmem_st_32x32b_x16(tDP + lane_off + c * 32, pk);
-      tmem_st_wait();
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(ds_full);
-    }
-    // ---- epilogue: dQ (already scaled through dS) -> bf16
-    mbar_wait(dq_done, 0);
-    tcgen05_fence_after();
-    uint32_t v[32];
-    tmem_ld_32x32b_x32(tDQ + lane_off + c * 32, v);
-    tmem_ld_wait();
-    if (q_idx < row_limit) {
-      if (!q_ok) {
-#pragma unroll
-        for (int t = 0; t < 32; ++t) v[t] = 0u;
-      }
-      store_bf16x32(p.dq + (long long)(tok0 + q_idx) * p.lddq + (long long)h * 128 + c * 32, v);
-    }
+    return;
   }
 
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tcgen05_fence_after();
-    tmem_dealloc<512>(tmem);
+  setmaxnreg_inc<232>();
+  const int c = wg - 1, ct = threadIdx.x - 128;
+  // ---- preamble: delta = rowsum(dO o O) from the swizzled TMA tiles (two [128 x 64] boxes, 16-byte chunks XOR row%8)
+  mbar_wait(q_full, 0);
+  {
+    const int r = ct & 127, hh = ct >> 7;
+    float part = 0.f;
+    const uint32_t off = (uint32_t)hh * 16384u + (uint32_t)r * 128u;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const uint32_t slot = (uint32_t)((i ^ (r & 7)) << 4);
+      const int4 a = *reinterpret_cast<const int4*>(base_ptr + BW_TILE + off + slot);          // dO
+      const int4 o = *reinterpret_cast<const int4*>(base_ptr + 5 * BW_TILE + off + slot);      // O (V stage 1)
+      const uint32_t ua[4] = {(uint32_t)a.x, (uint32_t)a.y, (uint32_t)a.z, (uint32_t)a.w};
+      const uint32_t uo[4] = {(uint32_t)o.x, (uint32_t)o.y, (uint32_t)o.z, (uint32_t)o.w};
+#pragma unroll
+      for (int t = 0; t < 4; ++t) {
+        const float2 x = unpack_bf16x2(ua[t]);
+        const float2 y = unpack_bf16x2(uo[t]);
+        part = fmaf(x.x, y.x, fmaf(x.y, y.y, part));
+      }
+    }
+    sRed[hh * 128 + r] = part;
   }
+  consumer_release(o_used);                                  // this warp no longer reads the O tile
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  if (ct < 128) {
+    const bool ok = q0 + ct < kv_len;
+    p.delta[stat0 + ct] = ok ? (sRed[ct] + sRed[128 + ct]) * p.scale : 0.f;
+    p.lse2[stat0 + ct] = ok ? p.lse[((long long)b * p.Hq + h) * p.T + q0 + ct] * kLog2e : 0.f;
+  }
+  const int g = ((threadIdx.x & 127) >> 5) * 16 + (lane >> 2), q2 = (lane & 3) * 2;
+  int q_idx[2];
+  bool q_ok[2];
+  float delta[2], lse2[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int r = c * 64 + g + 8 * i;
+    q_idx[i] = q0 + r;
+    q_ok[i] = q_idx[i] < kv_len;
+    delta[i] = q_ok[i] ? (sRed[r] + sRed[128 + r]) * p.scale : 0.f;
+    lse2[i] = q_ok[i] ? p.lse[((long long)b * p.Hq + h) * p.T + q_idx[i]] * kLog2e : 0.f;
+  }
+  const float sl2 = p.scale * kLog2e;
+  const uint32_t sQc = sQ + (uint32_t)c * 8192u, sdOc = sdO + (uint32_t)c * 8192u;
+  float dq[64];
+  for (int j = 0; j < n_tiles; ++j) {
+    const int bf = j & 1;
+    const uint32_t ph = (uint32_t)((j >> 1) & 1);
+    mbar_wait(bf ? k_full1 : k_full0, ph);
+    mbar_wait(bf ? v_full1 : v_full0, ph);
+#pragma unroll 1
+    for (int hf = 0; hf < 2; ++hf) {               // 64 keys at a time
+      float s[32], dp[32];
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        wgmma_m64n64_ss<0, 0>(s, desc_kmajor(sQc, k), desc_kmajor(sK[bf] + hf * 8192u, k), k != 0 ? 1u : 0u);
+        wgmma_m64n64_ss<0, 0>(dp, desc_kmajor(sdOc, k), desc_kmajor(sV[bf] + hf * 8192u, k), k != 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      // P = exp2(S * scale*log2e - lse2);  dS = P o (dP*scale - delta)
+      const int k0 = j * 128 + hf * 64;
+#pragma unroll
+      for (int t = 0; t < 32; ++t) {
+        const int i = (t >> 1) & 1;
+        const int col = k0 + (t >> 2) * 8 + q2 + (t & 1);
+        const bool ok = q_ok[i] && col <= q_idx[i] && col < kv_len;
+        const float pv = ok ? fast_exp2(fmaf(s[t], sl2, -lse2[i])) : 0.f;
+        s[t] = pv * fmaf(dp[t], p.scale, -delta[i]);
+      }
+      uint32_t da[4][4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) acc_to_a(s, k, da[k]);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_m64n128_rs<1>(dq, da[k], desc_mnmajor(sK[bf], hf * 4 + k), (j | hf | k) != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+    }
+    consumer_release(bf ? k_empty1 : k_empty0);
+    consumer_release(bf ? v_empty1 : v_empty0);
+  }
+  // ---- epilogue: dQ (already scaled through dS) -> bf16
+  bf16* d0 = p.dq + (long long)(tok0 + q_idx[0]) * p.lddq + (long long)h * 128;
+  bf16* d1 = p.dq + (long long)(tok0 + q_idx[1]) * p.lddq + (long long)h * 128;
+  store_acc_rows(d0, d1, q_idx[0] < row_limit, q_idx[1] < row_limit, q_ok[0], q_ok[1], dq, q2);
 }
 
 // =================================================================================================== kernel 2: dK, dV
+// One CTA = 64 keys. Warpgroup 1 accumulates dV, warpgroup 2 dK (both compute S^T and dP^T): the two 64 x 128 fp32
+// accumulators of one warpgroup would not fit its register budget next to the S^T / dP^T fragments.
 __global__ void __launch_bounds__(BW_THREADS, 1)
 flash_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                      const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do,
                      const __grid_constant__ CUtensorMap tmap_stat, BwdTcParams p) {
   extern __shared__ uint8_t smem_raw[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // grid = (Hkv*B, key tiles): CTAs are dispatched x-fastest, so ALL (head, batch) instances of the heaviest key tile
-  // (j = 0 sees every query tile) start first and the light tiles fill the tail (LPT-style schedule)
-  // (packed sequences: grid = (key-tile work list, kv heads))
-  const int jt = p.work_k ? p.work_k[blockIdx.x].y : (int)blockIdx.y;
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
+  // grid = (Hkv*B, 64-key tiles): CTAs are dispatched x-fastest, so ALL (head, batch) instances of the heaviest key tile
+  // (tile 0 sees every query tile) start first and the light tiles fill the tail (LPT-style schedule)
+  // (packed sequences: grid = (2 x key-tile work list, kv heads); the list names 128-key tiles)
+  const int jt = p.work_k ? 2 * p.work_k[blockIdx.x >> 1].y + (int)(blockIdx.x & 1) : (int)blockIdx.y;
   const int hk = p.work_k ? (int)blockIdx.y : (int)(blockIdx.x % p.Hkv);
-  const int b = p.work_k ? p.work_k[blockIdx.x].x : (int)(blockIdx.x / p.Hkv);
+  const int b = p.work_k ? p.work_k[blockIdx.x >> 1].x : (int)(blockIdx.x / p.Hkv);
   const int G = p.Hq / p.Hkv;
-  const int kv0 = jt * 128;
+  const int kv0 = jt * 64;
   const int kv_len = p.seqlens ? min(p.seqlens[b], p.T) : p.T;
   const int tok0 = p.seg_start ? p.seg_start[b] : b * p.T;
   const int row_limit = p.seg_start ? kv_len : p.T;
 
   if (kv0 >= kv_len) {   // the whole key tile is padding
-    for (int i = threadIdx.x; i < 128 * 16; i += BW_THREADS) {
+    for (int i = threadIdx.x; i < 64 * 16; i += BW_THREADS) {
       const int r = i >> 4, c = (i & 15) * 8;
       if (kv0 + r < row_limit) {
         *reinterpret_cast<int4*>(p.dk + (long long)(tok0 + kv0 + r) * p.lddk + (long long)hk * 128 + c) = make_int4(0, 0, 0, 0);
@@ -338,238 +262,129 @@ flash_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
     }
     return;
   }
-  const int qt_begin = jt;                                   // causal: query tiles at or after this key tile ...
+  const int qt_begin = kv0 / 128;                            // causal: query tiles of 128 at or after this key tile ...
   const int n_qt = (kv_len + 127) / 128 - qt_begin;          // ... that contain at least one real query
   const int n_it = n_qt * G;
 
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
-  const uint32_t sK = base, sV = base + BW_TILE;
+  const uint32_t sK = base, sV = base + BW_TILE;             // [64 keys x 64] boxes at +0 / +16 KB (the K-major layout)
   const uint32_t sQ[2] = {base + 2 * BW_TILE, base + 4 * BW_TILE};
   const uint32_t sdO[2] = {base + 3 * BW_TILE, base + 5 * BW_TILE};
-  float* sStat = reinterpret_cast<float*>(base_ptr + 6 * BW_TILE);   // [2 buffers][lse2 128 | delta 128]
+  const float* sStat = reinterpret_cast<const float*>(base_ptr + 6 * BW_TILE);   // [2 buffers][lse2 128 | delta 128]
   const uint32_t uStat = base + 6 * BW_TILE;
   const uint32_t bar = base + 6 * BW_TILE + 2048;
-  const uint32_t kv_full = bar, qdo_full0 = bar + 8, qdo_full1 = bar + 16, qdo_empty0 = bar + 24,
-                 qdo_empty1 = bar + 32, st_full = bar + 40, dp_full = bar + 48, p_full = bar + 56, ds_full = bar + 64,
-                 fin_full = bar + 72, tmem_slot = bar + 80, stat_empty0 = bar + 88, stat_empty1 = bar + 96;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(base_ptr + 6 * BW_TILE + 2048 + 80);
+  const uint32_t kv_full = bar, qdo_full0 = bar + 8, qdo_full1 = bar + 16, qdo_empty0 = bar + 24, qdo_empty1 = bar + 32;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_q);
     prefetch_tmap(&tmap_k);
     prefetch_tmap(&tmap_v);
     prefetch_tmap(&tmap_do);
-    for (int i = 0; i < 7; ++i) mbar_init(bar + 8 * i, 1);   // kv_full .. dp_full
-    mbar_init(p_full, 16);
-    mbar_init(ds_full, 16);
-    mbar_init(fin_full, 1);
-    mbar_init(stat_empty0, 16);   // the 16 elementwise warps have read the lse2 / delta rows of this buffer
-    mbar_init(stat_empty1, 16);
+    prefetch_tmap(&tmap_stat);
+    mbar_init(kv_full, 1);
+    mbar_init(qdo_full0, 1);
+    mbar_init(qdo_full1, 1);
+    mbar_init(qdo_empty0, 8);   // one arrive per consumer warp: Q, dO and the statistics rows of the buffer are read
+    mbar_init(qdo_empty1, 8);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<512>(tmem_slot);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem = *tmem_slot_ptr;
-  const uint32_t tST = tmem, tDPT = tmem + 128, tDV = tmem + 256, tDK = tmem + 384;
 
-  if (warp == 0 && lane == 0) {
+  if (wg == 0) {
     // ---------------------------------------------------------------- TMA producer
-    mbar_arrive_expect_tx(kv_full, 2 * BW_TILE);
-    tma_load_2d(sK, &tmap_k, kv_full, hk * 128, tok0 + kv0);
-    tma_load_2d(sK + 16384, &tmap_k, kv_full, hk * 128 + 64, tok0 + kv0);
-    tma_load_2d(sV, &tmap_v, kv_full, hk * 128, tok0 + kv0);
-    tma_load_2d(sV + 16384, &tmap_v, kv_full, hk * 128 + 64, tok0 + kv0);
-    for (int it = 0; it < n_it; ++it) {
-      const int buf = it & 1, use = it >> 1;
-      const int hq = hk * G + it / n_qt;
-      const int q0 = (qt_begin + it % n_qt) * 128;
-      const uint32_t full = buf ? qdo_full1 : qdo_full0, empty = buf ? qdo_empty1 : qdo_empty0;
-      mbar_wait(empty, (uint32_t)((use & 1) ^ 1));          // the MMAs that read Q / dO of this buffer have completed
-      // The statistics rows are read by the elementwise warps (generic proxy): their own barrier orders the overwrite
-      // directly (it is also implied by ds_full -> MMA thread -> commit on `empty`, a chain racecheck cannot follow).
-      mbar_wait(buf ? stat_empty1 : stat_empty0, (uint32_t)((use & 1) ^ 1));
-      mbar_arrive_expect_tx(full, 2 * BW_TILE + 1024);
-      tma_load_2d(sQ[buf], &tmap_q, full, hq * 128, tok0 + q0);
-      tma_load_2d(sQ[buf] + 16384, &tmap_q, full, hq * 128 + 64, tok0 + q0);
-      tma_load_2d(sdO[buf], &tmap_do, full, hq * 128, tok0 + q0);
-      tma_load_2d(sdO[buf] + 16384, &tmap_do, full, hq * 128 + 64, tok0 + q0);
-      // statistics rows of the workspace: [lse2 rows of all (b, head) | delta rows of all (b, head)], 128 values each
-      // (after the 64 KB of Q / dO: the first MMA of the iteration needs those, the statistics only its elementwise phase)
-      tma_load_2d(uStat + buf * 1024, &tmap_stat, full, q0, b * p.Hq + hq);
-      tma_load_2d(uStat + buf * 1024 + 512, &tmap_stat, full, q0, (p.B + b) * p.Hq + hq);
-    }
-  } else if (warp == 1 && lane == 0) {
-    // ---------------------------------------------------------------- MMA issuer
-    auto issue_st = [&](int it) {
-      const int buf = it & 1;
-#pragma unroll
-      for (int k = 0; k < 8; ++k)
-        umma_bf16_ss(tST, desc_kmajor(sK, k), desc_kmajor(sQ[buf], k), kIdescKK, k != 0 ? 1u : 0u);
-      umma_commit(st_full);
-    };
-    auto issue_dpt = [&](int it) {
-      const int buf = it & 1;
-#pragma unroll
-      for (int k = 0; k < 8; ++k)
-        umma_bf16_ss(tDPT, desc_kmajor(sV, k), desc_kmajor(sdO[buf], k), kIdescKK, k != 0 ? 1u : 0u);
-      umma_commit(dp_full);
-    };
-    mbar_wait(kv_full, 0);
-    mbar_wait(qdo_full0, 0);
-    tcgen05_fence_after();
-    issue_st(0);
-    issue_dpt(0);
-    for (int it = 0; it < n_it; ++it) {
-      const int buf = it & 1;
-      const uint32_t ph = (uint32_t)(it & 1);
-      mbar_wait(p_full, ph);                              // P^T_it packed into the S^T columns
-      tcgen05_fence_after();
-#pragma unroll
-      for (int k = 0; k < 8; ++k)
-        umma_bf16_ts(tDV, tST + packed_col(k), desc_mnmajor(sdO[buf], k), kIdescBmn, (it | k) != 0 ? 1u : 0u);
-      if (it + 1 < n_it) {
-        mbar_wait((it + 1) & 1 ? qdo_full1 : qdo_full0, (uint32_t)(((it + 1) >> 1) & 1));
-        tcgen05_fence_after();
-        issue_st(it + 1);                                 // overwrites P^T_it: issued after the dV MMAs that read it
-      }
-      mbar_wait(ds_full, ph);                             // dS^T_it packed into the dP^T columns
-      tcgen05_fence_after();
-#pragma unroll
-      for (int k = 0; k < 8; ++k)
-        umma_bf16_ts(tDK, tDPT + packed_col(k), desc_mnmajor(sQ[buf], k), kIdescBmn, (it | k) != 0 ? 1u : 0u);
-      umma_commit(buf ? qdo_empty1 : qdo_empty0);         // every product of this iteration has read Q / dO
-      if (it + 1 < n_it) issue_dpt(it + 1);               // overwrites dS^T_it: issued after the dK MMAs that read it
-    }
-    umma_commit(fin_full);
-  } else if (warp >= 2) {
-    // ---------------------------------------------------------------- elementwise: thread = key row r x 32 query columns
-    const int quad = warp & 3;
-    const int c = (warp - 2) >> 2;
-    const int r = quad * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(quad * 32) << 16;
-    const int key_idx = kv0 + r;
-    const bool key_ok = key_idx < kv_len;
-    const float sl2 = p.scale * kLog2e;
-    for (int it = 0; it < n_it; ++it) {
-      const uint32_t ph = (uint32_t)(it & 1);
-      const int q0 = (qt_begin + it % n_qt) * 128;
-      const int sbuf = it & 1;
-      const float* sLse = sStat + sbuf * 256 + c * 32;      // lse2 / delta of this thread's 32 query columns
-      const float* sDelta = sLse + 128;
-      mbar_wait(sbuf ? qdo_full1 : qdo_full0, (uint32_t)((it >> 1) & 1));   // statistics arrive with the Q/dO transaction
-      // ---- phase 1: P^T = exp2(S^T * scale*log2e - lse2[q])
-      mbar_wait(st_full, ph);
-      tcgen05_fence_after();
-      uint32_t s0[16], s1[16];
-      tmem_ld_32x32b_x16(tST + lane_off + c * 32, s0);
-      tmem_ld_32x32b_x16(tST + lane_off + c * 32 + 16, s1);
-      tmem_ld_wait();
-      const bool fast = key_ok && (q0 >= kv0 + 127) && (q0 + 128 <= kv_len);   // no causal / length edge in this tile
-      if (fast) {
-#pragma unroll
-        for (int t = 0; t < 16; t += 4) {
-          const float4 l0 = *reinterpret_cast<const float4*>(sLse + t);
-          const float4 l1 = *reinterpret_cast<const float4*>(sLse + 16 + t);
-          s0[t] = __float_as_uint(fast_exp2(fmaf(__uint_as_float(s0[t]), sl2, -l0.x)));
-          s0[t + 1] = __float_as_uint(fast_exp2(fmaf(__uint_as_float(s0[t + 1]), sl2, -l0.y)));
-          s0[t + 2] = __float_as_uint(fast_exp2(fmaf(__uint_as_float(s0[t + 2]), sl2, -l0.z)));
-          s0[t + 3] = __float_as_uint(fast_exp2(fmaf(__uint_as_float(s0[t + 3]), sl2, -l0.w)));
-          s1[t] = __float_as_uint(fast_exp2(fmaf(__uint_as_float(s1[t]), sl2, -l1.x)));
-          s1[t + 1] = __float_as_uint(fast_exp2(fmaf(__uint_as_float(s1[t + 1]), sl2, -l1.y)));
-          s1[t + 2] = __float_as_uint(fast_exp2(fmaf(__uint_as_float(s1[t + 2]), sl2, -l1.z)));
-          s1[t + 3] = __float_as_uint(fast_exp2(fmaf(__uint_as_float(s1[t + 3]), sl2, -l1.w)));
-        }
-      } else {
-#pragma unroll
-        for (int t = 0; t < 16; ++t) {
-          const int qa = q0 + c * 32 + t, qb = qa + 16;
-          const bool ok0 = key_ok && (qa < kv_len) && (key_idx <= qa);
-          const bool ok1 = key_ok && (qb < kv_len) && (key_idx <= qb);
-          s0[t] = ok0 ? __float_as_uint(fast_exp2(fmaf(__uint_as_float(s0[t]), sl2, -sLse[t]))) : 0u;
-          s1[t] = ok1 ? __float_as_uint(fast_exp2(fmaf(__uint_as_float(s1[t]), sl2, -sLse[16 + t]))) : 0u;
-        }
-      }
-      {
-        uint32_t pk[16];
-#pragma unroll
-        for (int t = 0; t < 16; t += 2) {
-          pk[t >> 1] = pack_bf16x2(__uint_as_float(s0[t]), __uint_as_float(s0[t + 1]));
-          pk[8 + (t >> 1)] = pack_bf16x2(__uint_as_float(s1[t]), __uint_as_float(s1[t + 1]));
-        }
-        tmem_st_32x32b_x16(tST + lane_off + c * 32, pk);
-      }
-      tmem_st_wait();
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-      // ---- phase 2: dS^T = P^T o (dP^T*scale - delta[q])   (P is exactly 0 wherever the mask applies, and the
-      // statistics of masked columns are finite, so no second mask is needed)
-      mbar_wait(dp_full, ph);
-      tcgen05_fence_after();
-      {
-        uint32_t pk[16], d[16];
-        tmem_ld_32x32b_x16(tDPT + lane_off + c * 32, d);
-        tmem_ld_wait();
-#pragma unroll
-        for (int t = 0; t < 16; t += 2)
-          pk[t >> 1] = pack_bf16x2(__uint_as_float(s0[t]) * fmaf(__uint_as_float(d[t]), p.scale, -sDelta[t]),
-                                   __uint_as_float(s0[t + 1]) * fmaf(__uint_as_float(d[t + 1]), p.scale, -sDelta[t + 1]));
-        tmem_ld_32x32b_x16(tDPT + lane_off + c * 32 + 16, d);
-        tmem_ld_wait();
-#pragma unroll
-        for (int t = 0; t < 16; t += 2)
-          pk[8 + (t >> 1)] =
-              pack_bf16x2(__uint_as_float(s1[t]) * fmaf(__uint_as_float(d[t]), p.scale, -sDelta[16 + t]),
-                          __uint_as_float(s1[t + 1]) * fmaf(__uint_as_float(d[t + 1]), p.scale, -sDelta[16 + t + 1]));
-        tmem_st_32x32b_x16(tDPT + lane_off + c * 32, pk);
-      }
-      tmem_st_wait();
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(ds_full);
-        mbar_arrive(sbuf ? stat_empty1 : stat_empty0);
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      mbar_arrive_expect_tx(kv_full, 4 * 64 * 128);
+      tma_load_2d(sK, &tmap_k, kv_full, hk * 128, tok0 + kv0);
+      tma_load_2d(sK + 16384, &tmap_k, kv_full, hk * 128 + 64, tok0 + kv0);
+      tma_load_2d(sV, &tmap_v, kv_full, hk * 128, tok0 + kv0);
+      tma_load_2d(sV + 16384, &tmap_v, kv_full, hk * 128 + 64, tok0 + kv0);
+      for (int it = 0; it < n_it; ++it) {
+        const int buf = it & 1, use = it >> 1;
+        const int hq = hk * G + it / n_qt;
+        const int q0 = (qt_begin + it % n_qt) * 128;
+        const uint32_t full = buf ? qdo_full1 : qdo_full0, empty = buf ? qdo_empty1 : qdo_empty0;
+        mbar_wait(empty, (uint32_t)((use & 1) ^ 1));
+        mbar_arrive_expect_tx(full, 2 * BW_TILE + 1024);
+        tma_load_2d(sQ[buf], &tmap_q, full, hq * 128, tok0 + q0);
+        tma_load_2d(sQ[buf] + 16384, &tmap_q, full, hq * 128 + 64, tok0 + q0);
+        tma_load_2d(sdO[buf], &tmap_do, full, hq * 128, tok0 + q0);
+        tma_load_2d(sdO[buf] + 16384, &tmap_do, full, hq * 128 + 64, tok0 + q0);
+        // statistics rows of the workspace: [lse2 rows of all (b, head) | delta rows of all (b, head)], 128 values each
+        tma_load_2d(uStat + buf * 1024, &tmap_stat, full, q0, b * p.Hq + hq);
+        tma_load_2d(uStat + buf * 1024 + 512, &tmap_stat, full, q0, (p.B + b) * p.Hq + hq);
       }
     }
-    // ---- final: dK (already scaled through dS) and dV
-    mbar_wait(fin_full, 0);
-    tcgen05_fence_after();
-    // (tcgen05.ld is .sync.aligned: every lane of the warp executes it; only the global stores are predicated)
-    const bool row_ok = key_idx < row_limit;
-    {
-      uint32_t a[32];
-      tmem_ld_32x32b_x32(tDK + lane_off + c * 32, a);
-      tmem_ld_wait();
-      if (!key_ok) {
-#pragma unroll
-        for (int t = 0; t < 32; ++t) a[t] = 0u;
-      }
-      if (row_ok) store_bf16x32(p.dk + (long long)(tok0 + key_idx) * p.lddk + (long long)hk * 128 + c * 32, a);
-      tmem_ld_32x32b_x32(tDV + lane_off + c * 32, a);
-      tmem_ld_wait();
-      if (!key_ok) {
-#pragma unroll
-        for (int t = 0; t < 32; ++t) a[t] = 0u;
-      }
-      if (row_ok) store_bf16x32(p.dv + (long long)(tok0 + key_idx) * p.lddv + (long long)hk * 128 + c * 32, a);
-    }
+    return;
   }
 
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tcgen05_fence_after();
-    tmem_dealloc<512>(tmem);
+  setmaxnreg_inc<232>();
+  const bool is_dk = wg == 2;
+  const int g = ((threadIdx.x & 127) >> 5) * 16 + (lane >> 2), q2 = (lane & 3) * 2;
+  int key_idx[2];
+  bool key_ok[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    key_idx[i] = kv0 + g + 8 * i;
+    key_ok[i] = key_idx[i] < kv_len;
   }
+  const float sl2 = p.scale * kLog2e;
+  float acc[64];                                   // dV (warpgroup 1) or dK (warpgroup 2)
+  mbar_wait(kv_full, 0);
+  for (int it = 0; it < n_it; ++it) {
+    const int buf = it & 1;
+    const int q0 = (qt_begin + it % n_qt) * 128;
+    mbar_wait(buf ? qdo_full1 : qdo_full0, (uint32_t)((it >> 1) & 1));
+    const float* sLse = sStat + buf * 256;
+    const float* sDelta = sLse + 128;
+#pragma unroll 1
+    for (int hf = 0; hf < 2; ++hf) {               // 64 queries at a time
+      float s[32], dp[32];
+      uint32_t fa[4][4];
+      // both warpgroups issue the same products (dP^T is only used by the dK one): wgmma in a warpgroup-divergent branch
+      // would make ptxas serialise every wgmma of the kernel, and the dK warpgroup sets the pace either way
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        wgmma_m64n64_ss<0, 0>(s, desc_kmajor(sK, k), desc_kmajor(sQ[buf] + hf * 8192u, k), k != 0 ? 1u : 0u);
+        wgmma_m64n64_ss<0, 0>(dp, desc_kmajor(sV, k), desc_kmajor(sdO[buf] + hf * 8192u, k), k != 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      // P^T = exp2(S^T * scale*log2e - lse2[q]);  dK warpgroup: dS^T = P^T o (dP^T*scale - delta[q])
+#pragma unroll
+      for (int t = 0; t < 32; ++t) {
+        const int i = (t >> 1) & 1;
+        const int ql = hf * 64 + (t >> 2) * 8 + q2 + (t & 1);   // query column within the 128-query tile
+        const bool ok = key_ok[i] && (q0 + ql < kv_len) && (key_idx[i] <= q0 + ql);
+        const float pv = ok ? fast_exp2(fmaf(s[t], sl2, -sLse[ql])) : 0.f;
+        s[t] = is_dk ? pv * fmaf(dp[t], p.scale, -sDelta[ql]) : pv;
+      }
+#pragma unroll
+      for (int k = 0; k < 4; ++k) acc_to_a(s, k, fa[k]);
+      // dV += P^T dO  /  dK += dS^T Q   (B MN-major: query rows of the tile are the contraction)
+      const uint32_t sB = is_dk ? sQ[buf] : sdO[buf];
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_m64n128_rs<1>(acc, fa[k], desc_mnmajor(sB, hf * 4 + k), (it | hf | k) != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+    }
+    consumer_release(buf ? qdo_empty1 : qdo_empty0);
+  }
+  // ---- final: dK (already scaled through dS) or dV
+  bf16* dst = is_dk ? p.dk : p.dv;
+  const long long ld = is_dk ? p.lddk : p.lddv;
+  store_acc_rows(dst + (long long)(tok0 + key_idx[0]) * ld + (long long)hk * 128,
+                 dst + (long long)(tok0 + key_idx[1]) * ld + (long long)hk * 128, key_idx[0] < row_limit,
+                 key_idx[1] < row_limit, key_ok[0], key_ok[1], acc, q2);
 }
 
 }  // namespace
 
-// Workspace of the tcgen05 backward: lse*log2e and delta, [B, Hq, Tp] fp32 each (Tp = T rounded up to 128).
+// Workspace of the backward: lse*log2e and delta, [B, Hq, Tp] fp32 each (Tp = T rounded up to 128).
 MM_API long long mm_attn_bwd_tc_workspace_bytes(int B, int T, int Hq) {
   const long long Tp = ((long long)T + 127) / 128 * 128;
   return 2 * (((long long)B * Hq * Tp * 4 + 255) / 256 * 256);
@@ -593,7 +408,7 @@ int launch_bwd_tc(const void* q, const void* k, const void* v, const void* o, co
                "mm_attn_bwd_tc: 16-byte alignment required");
   const int Tp = (T + 127) / 128 * 128;
   const long long stat_bytes = ((long long)B * Hq * Tp * 4 + 255) / 256 * 256;
-  CUtensorMap tq, tk, tv, tdo, to, tstat;
+  CUtensorMap tq, tk, tv, tdo, to, tstat, tk64, tv64;
   int rc;
   MM_CHECK_ARG(stat_bytes == (long long)B * Hq * Tp * 4, "mm_attn_bwd_tc: statistics rows must be contiguous");
   if ((rc = mm_attn_make_tmap_stats(&tstat, reinterpret_cast<const float*>(workspace), Tp, 2LL * B * Hq))) return rc;
@@ -602,6 +417,8 @@ int launch_bwd_tc(const void* q, const void* k, const void* v, const void* o, co
   if ((rc = mm_attn_make_tmap_rows(&tv, v, (long long)Hkv * 128, total_rows, ldv))) return rc;
   if ((rc = mm_attn_make_tmap_rows(&tdo, dout, (long long)Hq * 128, total_rows, lddo))) return rc;
   if ((rc = mm_attn_make_tmap_rows(&to, o, (long long)Hq * 128, total_rows, ldo))) return rc;
+  if ((rc = mm_attn_make_tmap_rows(&tk64, k, (long long)Hkv * 128, total_rows, ldk, 64))) return rc;
+  if ((rc = mm_attn_make_tmap_rows(&tv64, v, (long long)Hkv * 128, total_rows, ldv, 64))) return rc;
   static std::once_flag once;
   static cudaError_t err = cudaSuccess;
   std::call_once(once, [&] {
@@ -620,17 +437,17 @@ int launch_bwd_tc(const void* q, const void* k, const void* v, const void* o, co
   p.B = B; p.T = T; p.Tp = Tp; p.Hq = Hq; p.Hkv = Hkv; p.scale = scale;
   const int n_tiles = (T + 127) / 128;
   const dim3 grid_q = work_q ? dim3(n_work_q, Hq, 1) : dim3(n_tiles, Hq, B);
-  const dim3 grid_k = work_k ? dim3(n_work_k, Hkv, 1) : dim3(Hkv * B, n_tiles, 1);
+  const dim3 grid_k = work_k ? dim3(2 * n_work_k, Hkv, 1) : dim3(Hkv * B, 2 * n_tiles, 1);
   flash_bwd_dq_kernel<<<grid_q, BW_THREADS, BW_SMEM, stream>>>(tq, tk, tv, tdo, to, p);
   MM_CHECK_LAUNCH();
-  flash_bwd_dkv_kernel<<<grid_k, BW_THREADS, BW_SMEM, stream>>>(tq, tk, tv, tdo, tstat, p);
+  flash_bwd_dkv_kernel<<<grid_k, BW_THREADS, BW_SMEM, stream>>>(tq, tk64, tv64, tdo, tstat, p);
   MM_CHECK_LAUNCH();
   return MM_OK;
 }
 
 }  // namespace
 
-// tcgen05 flash-attention backward; same argument meaning as mm_attn_bwd (workspace from mm_attn_bwd_tc_workspace_bytes).
+// wgmma flash-attention backward; same argument meaning as mm_attn_bwd (workspace from mm_attn_bwd_tc_workspace_bytes).
 MM_API int mm_attn_bwd_tc(const void* q, const void* k, const void* v, const void* o, const void* dout,
                           const float* lse, void* dq, void* dk, void* dv, const int* seqlens, long long ldq,
                           long long ldk, long long ldv, long long ldo, long long lddo, long long lddq,

@@ -1,16 +1,13 @@
-// metamorph_b200 — flash attention FORWARD on 5th-gen tensor cores (tcgen05 + TMEM + TMA), head_dim 128.
+// metamorph_b200 — flash attention FORWARD on Hopper tensor cores (wgmma + TMA + mbarrier), head_dim 128.
 // (SURVEY.md K12: LLaMA causal GQA attention, HF modeling_llama.py:199-220 / SDPA in 4.45.)
 //
 // One CTA = 128 query rows of one (batch, q-head), 1 CTA/SM; K/V tiles of 128 keys stream through a double-buffered
 // TMA ring.
-//   warp 0      : TMA producer
-//   warp 1      : MMA issuer     S_j = Q K_j^T (SS, both K-major) -> TMEM, double-buffered so that the tensor core
-//                                computes S_{j+1} while the CUDA cores run softmax_j;
-//                                O += P_j V_j (TS: A = P in TMEM, B = V MN-major from the same TMA tile)
-//   warps 2..17 : softmax        warp -> (TMEM lane quadrant, 32-column chunk): one TMEM pass over S per tile (values
-//                                stay in registers), one named barrier per tile to exchange the row maxima of the four
-//                                column chunks, P written back to TMEM as packed bf16 over the consumed S columns,
-//                                lazy O rescale (only when the running max grows by > 2^8, FA4-style).
+//   warpgroup 0, one thread : TMA producer
+//   warpgroups 1, 2         : 64 query rows each. S_j = Q K_j^T (wgmma, both operands K-major in shared memory) lands
+//                             in registers; the online softmax runs on the accumulator fragments (a row's 128 scores
+//                             are spread over the 4 lanes of a quad); P_j is packed to bf16 in place and is the
+//                             register A operand of O += P_j V_j (V MN-major from the same TMA tile).
 // The backward lives in attention_bwd_tc.cu.
 #include "attention_tc.cuh"
 
@@ -33,29 +30,22 @@ struct TcFwdParams {
   int causal;
 };
 
-constexpr int TC2_THREADS = 576;
-constexpr int TC2_SMEM = 5 * TC_TILE_BYTES + 2 * 4 * 128 * 4 + 4 * 128 * 4 + 256 + 1024;
+constexpr int TC_THREADS = 384;
+constexpr int TC_SMEM = 5 * TC_TILE_BYTES + 256 + 1024;
 
-__global__ void __launch_bounds__(TC2_THREADS, 1)
-flash_fwd_tc2_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                     const __grid_constant__ CUtensorMap tmap_v, TcFwdParams p) {
+__global__ void __launch_bounds__(TC_THREADS, 1)
+flash_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                       const __grid_constant__ CUtensorMap tmap_v, TcFwdParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
   const uint32_t sQ = base;
   const uint32_t sK[2] = {base + TC_TILE_BYTES, base + 2 * TC_TILE_BYTES};
   const uint32_t sV[2] = {base + 3 * TC_TILE_BYTES, base + 4 * TC_TILE_BYTES};
-  float* sMax = reinterpret_cast<float*>(base_ptr + 5 * TC_TILE_BYTES);   // [2][4][128]
-  float* sSum = sMax + 2 * 4 * 128;                                       // [4][128]
-  const uint32_t bar = base + 5 * TC_TILE_BYTES + 2 * 4 * 128 * 4 + 4 * 128 * 4;
+  const uint32_t bar = base + 5 * TC_TILE_BYTES;
   const uint32_t q_full = bar, k_full0 = bar + 8, k_full1 = bar + 16, k_empty0 = bar + 24, k_empty1 = bar + 32,
-                 v_full0 = bar + 40, v_full1 = bar + 48, v_empty0 = bar + 56, v_empty1 = bar + 64,
-                 s_full0 = bar + 72, s_full1 = bar + 80, p_full0 = bar + 88, p_full1 = bar + 96,
-                 o_done = bar + 104, tmem_slot = bar + 112;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(
-      base_ptr + 5 * TC_TILE_BYTES + 2 * 4 * 128 * 4 + 4 * 128 * 4 + 112);
+                 v_full0 = bar + 40, v_full1 = bar + 48, v_empty0 = bar + 56, v_empty1 = bar + 64;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   // padded batch: grid = (query tiles, heads, sequences), heavy (late) tiles first; packed sequences (SURVEY 8f N2):
   // grid.x walks a host-built list of the (sequence, query tile) pairs that exist, one launch for all segments
   const int qt = p.work ? p.work[blockIdx.x].y : (int)gridDim.x - 1 - (int)blockIdx.x;
@@ -69,184 +59,129 @@ flash_fwd_tc2_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
   const int tok0 = p.seg_start ? p.seg_start[b] : b * p.T;
   const int row_limit = p.seg_start ? kv_len : p.T;   // packed: rows past the sequence belong to the next one
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_q);
     prefetch_tmap(&tmap_k);
     prefetch_tmap(&tmap_v);
-    for (int i = 0; i < 9; ++i) mbar_init(bar + 8 * i, 1);   // q_full .. v_empty1
-    mbar_init(s_full0, 1);
-    mbar_init(s_full1, 1);
-    mbar_init(p_full0, 16);
-    mbar_init(p_full1, 16);
-    mbar_init(o_done, 1);
+    mbar_init(q_full, 1);
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(k_full0 + 8 * i, 1);
+      mbar_init(v_full0 + 8 * i, 1);
+      mbar_init(k_empty0 + 8 * i, 8);   // one arrive per consumer warp
+      mbar_init(v_empty0 + 8 * i, 8);
+    }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<512>(tmem_slot);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem = *tmem_slot_ptr;
-  const uint32_t tSb[2] = {tmem, tmem + 128};
-  const uint32_t tO = tmem + 256;
 
-  if (warp == 0 && lane == 0) {
-    if (n_tiles > 0) {
-      mbar_arrive_expect_tx(q_full, TC_TILE_BYTES);
-      tma_load_2d(sQ, &tmap_q, q_full, h * TC_D, tok0 + q0);
-      tma_load_2d(sQ + 16384, &tmap_q, q_full, h * TC_D + 64, tok0 + q0);
-    }
-    for (int j = 0; j < n_tiles; ++j) {
-      const int bf = j & 1;
-      const uint32_t ph = (uint32_t)((j >> 1) & 1);
-      mbar_wait(bf ? k_empty1 : k_empty0, ph ^ 1);
-      mbar_arrive_expect_tx(bf ? k_full1 : k_full0, TC_TILE_BYTES);
-      tma_load_2d(sK[bf], &tmap_k, bf ? k_full1 : k_full0, hk * TC_D, tok0 + j * TC_BC);
-      tma_load_2d(sK[bf] + 16384, &tmap_k, bf ? k_full1 : k_full0, hk * TC_D + 64, tok0 + j * TC_BC);
-      mbar_wait(bf ? v_empty1 : v_empty0, ph ^ 1);
-      mbar_arrive_expect_tx(bf ? v_full1 : v_full0, TC_TILE_BYTES);
-      tma_load_2d(sV[bf], &tmap_v, bf ? v_full1 : v_full0, hk * TC_D, tok0 + j * TC_BC);
-      tma_load_2d(sV[bf] + 16384, &tmap_v, bf ? v_full1 : v_full0, hk * TC_D + 64, tok0 + j * TC_BC);
-    }
-  } else if (warp == 1 && lane == 0) {
-    const uint32_t idesc_s = (1u << 4) | (1u << 7) | (1u << 10) | (uint32_t(TC_BC >> 3) << 17) |
-                             (uint32_t(TC_BR >> 4) << 24);
-    const uint32_t idesc_o = idesc_s | (1u << 16);
-    auto issue_s = [&](int j) {
-      const int bf = j & 1;
-      mbar_wait(bf ? k_full1 : k_full0, (uint32_t)((j >> 1) & 1));
-      tcgen05_fence_after();
-#pragma unroll
-      for (int k = 0; k < TC_D / 16; ++k)
-        umma_bf16_ss(tSb[bf], desc_kmajor(sQ, k), desc_kmajor(sK[bf], k), idesc_s, k != 0 ? 1u : 0u);
-      umma_commit(bf ? k_empty1 : k_empty0);
-      umma_commit(bf ? s_full1 : s_full0);
-    };
-    if (n_tiles > 0) {
-      mbar_wait(q_full, 0);
-      issue_s(0);
-    }
-    for (int j = 0; j < n_tiles; ++j) {
-      const int bf = j & 1;
-      const uint32_t ph = (uint32_t)((j >> 1) & 1);
-      if (j + 1 < n_tiles) {
-        // S buffer (j+1)&1 last held P_{j-1}: make sure PV_{j-1} has retired before overwriting it
-        if (j >= 1) mbar_wait(o_done, (uint32_t)((j - 1) & 1));
-        issue_s(j + 1);
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      if (n_tiles > 0) {
+        mbar_arrive_expect_tx(q_full, TC_TILE_BYTES);
+        tma_load_2d(sQ, &tmap_q, q_full, h * TC_D, tok0 + q0);
+        tma_load_2d(sQ + 16384, &tmap_q, q_full, h * TC_D + 64, tok0 + q0);
       }
-      mbar_wait(bf ? p_full1 : p_full0, ph);
-      mbar_wait(bf ? v_full1 : v_full0, ph);
-      tcgen05_fence_after();
-#pragma unroll
-      for (int k = 0; k < TC_BC / 16; ++k)
-        umma_bf16_ts(tO, tSb[bf] + (uint32_t)k * 8u, desc_mnmajor(sV[bf], k), idesc_o, (j | k) != 0 ? 1u : 0u);
-      umma_commit(bf ? v_empty1 : v_empty0);
-      umma_commit(o_done);
-    }
-  } else if (warp >= 2) {
-    const int quad = warp & 3;
-    const int c = (warp - 2) >> 2;
-    const int r = quad * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(quad * 32) << 16;
-    const int row = q0 + r;
-    const float sl2 = p.scale * kLog2e;
-    float m_used = -INFINITY, l_part = 0.f;
-    for (int j = 0; j < n_tiles; ++j) {
-      const int bf = j & 1;
-      const uint32_t ph = (uint32_t)((j >> 1) & 1);
-      mbar_wait(bf ? s_full1 : s_full0, ph);
-      tcgen05_fence_after();
-      const int c0 = j * TC_BC + c * 32;
-      const bool need_mask = (j * TC_BC + TC_BC > kv_len) || (p.causal && j * TC_BC + TC_BC - 1 > q0);
-      uint32_t v[32];
-      tmem_ld_32x32b_x32(tSb[bf] + lane_off + c * 32, v);
-      tmem_ld_wait();
-      float mx = -INFINITY;
-      if (need_mask) {
-#pragma unroll
-        for (int t = 0; t < 32; ++t) {
-          const int col = c0 + t;
-          const bool ok = (col < kv_len) && (!p.causal || col <= row);
-          const float x = ok ? __uint_as_float(v[t]) : -INFINITY;
-          v[t] = __float_as_uint(x);
-          mx = fmaxf(mx, x);
-        }
-      } else {
-#pragma unroll
-        for (int t = 0; t < 32; ++t) mx = fmaxf(mx, __uint_as_float(v[t]));
+      for (int j = 0; j < n_tiles; ++j) {
+        const int bf = j & 1;
+        const uint32_t ph = (uint32_t)((j >> 1) & 1);
+        mbar_wait(bf ? k_empty1 : k_empty0, ph ^ 1);
+        mbar_arrive_expect_tx(bf ? k_full1 : k_full0, TC_TILE_BYTES);
+        tma_load_2d(sK[bf], &tmap_k, bf ? k_full1 : k_full0, hk * TC_D, tok0 + j * TC_BC);
+        tma_load_2d(sK[bf] + 16384, &tmap_k, bf ? k_full1 : k_full0, hk * TC_D + 64, tok0 + j * TC_BC);
+        mbar_wait(bf ? v_empty1 : v_empty0, ph ^ 1);
+        mbar_arrive_expect_tx(bf ? v_full1 : v_full0, TC_TILE_BYTES);
+        tma_load_2d(sV[bf], &tmap_v, bf ? v_full1 : v_full0, hk * TC_D, tok0 + j * TC_BC);
+        tma_load_2d(sV[bf] + 16384, &tmap_v, bf ? v_full1 : v_full0, hk * TC_D + 64, tok0 + j * TC_BC);
       }
-      float* mrow = sMax + (j & 1) * 512;
-      mrow[c * 128 + r] = mx;
-      asm volatile("bar.sync 1, 512;" ::: "memory");   // all S loads done (P may alias) + maxima visible
-      mx = fmaxf(fmaxf(mrow[r], mrow[128 + r]), fmaxf(mrow[256 + r], mrow[384 + r])) * sl2;
-      const bool grow = (j > 0) && (mx > m_used + 8.f);
-      if (j == 0) m_used = mx;
-      if (__any_sync(0xffffffffu, grow)) {
-        mbar_wait(o_done, (uint32_t)((j - 1) & 1));
-        tcgen05_fence_after();
-        const float m_new = fmaxf(m_used, mx);
-        const float f = (m_new == -INFINITY) ? 1.f : fast_exp2(m_used - m_new);
-        l_part *= f;
-        m_used = m_new;
-        uint32_t o[32];
-        tmem_ld_32x32b_x32(tO + lane_off + c * 32, o);
-        tmem_ld_wait();
-#pragma unroll
-        for (int t = 0; t < 32; ++t) o[t] = __float_as_uint(__uint_as_float(o[t]) * f);
-        tmem_st_32x32b_x32(tO + lane_off + c * 32, o);
-      }
-      const float m_eff = (m_used == -INFINITY) ? 0.f : m_used;
-      uint32_t pk[16];
-#pragma unroll
-      for (int t = 0; t < 32; t += 2) {
-        const float e0 = fast_exp2(fmaf(__uint_as_float(v[t]), sl2, -m_eff));      // masked: exp2(-inf) = 0
-        const float e1 = fast_exp2(fmaf(__uint_as_float(v[t + 1]), sl2, -m_eff));
-        l_part += e0 + e1;
-        pk[t >> 1] = pack_bf16x2(e0, e1);
-      }
-      tmem_st_32x32b_x16(tSb[bf] + lane_off + c * 16, pk);
-      tmem_st_wait();
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bf ? p_full1 : p_full0);
     }
-    // epilogue: combine the four partial row sums, normalise, store
-    sSum[c * 128 + r] = l_part;
-    asm volatile("bar.sync 1, 512;" ::: "memory");
-    const float l_sum = sSum[r] + sSum[128 + r] + sSum[256 + r] + sSum[384 + r];
-    float inv = 0.f;
-    uint32_t o[32];
-    if (n_tiles > 0) {
-      mbar_wait(o_done, (uint32_t)((n_tiles - 1) & 1));
-      tcgen05_fence_after();
-      inv = l_sum > 0.f ? 1.f / l_sum : 0.f;
-      tmem_ld_32x32b_x32(tO + lane_off + c * 32, o);
-      tmem_ld_wait();
-    } else {
-#pragma unroll
-      for (int t = 0; t < 32; ++t) o[t] = 0u;
-    }
-    if (row < row_limit) {
-      bf16* orow = p.o + (long long)(tok0 + row) * p.ldo + (long long)h * TC_D + c * 32;
-#pragma unroll
-      for (int t = 0; t < 32; t += 8) {
-        int4 w;
-        w.x = pack_bf16x2(__uint_as_float(o[t]) * inv, __uint_as_float(o[t + 1]) * inv);
-        w.y = pack_bf16x2(__uint_as_float(o[t + 2]) * inv, __uint_as_float(o[t + 3]) * inv);
-        w.z = pack_bf16x2(__uint_as_float(o[t + 4]) * inv, __uint_as_float(o[t + 5]) * inv);
-        w.w = pack_bf16x2(__uint_as_float(o[t + 6]) * inv, __uint_as_float(o[t + 7]) * inv);
-        *reinterpret_cast<int4*>(orow + t) = w;
-      }
-      if (c == 0 && p.lse != nullptr)
-        p.lse[((long long)b * p.Hq + h) * p.T + row] = l_sum > 0.f ? (m_used + log2f(l_sum)) / kLog2e : -INFINITY;
-    }
+    return;
   }
 
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tcgen05_fence_after();
-    tmem_dealloc<512>(tmem);
+  setmaxnreg_inc<232>();
+  const int c = wg - 1;
+  const int g = ((threadIdx.x & 127) >> 5) * 16 + (lane >> 2), q2 = (lane & 3) * 2;
+  const int rows[2] = {q0 + c * 64 + g, q0 + c * 64 + g + 8};   // the two query rows of this thread
+  const float sl2 = p.scale * kLog2e;
+  const uint32_t sQc = sQ + (uint32_t)c * 8192u;                  // this warpgroup's 64 rows of the Q tile
+  float o[64], sacc[64];
+  float m_run[2] = {-INFINITY, -INFINITY}, l_part[2] = {0.f, 0.f};
+  if (n_tiles > 0) mbar_wait(q_full, 0);
+  for (int j = 0; j < n_tiles; ++j) {
+    const int bf = j & 1;
+    const uint32_t ph = (uint32_t)((j >> 1) & 1);
+    mbar_wait(bf ? k_full1 : k_full0, ph);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < TC_D / 16; ++k)
+      wgmma_m64n128_ss<0, 0>(sacc, desc_kmajor(sQc, k), desc_kmajor(sK[bf], k), k != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    consumer_release(bf ? k_empty1 : k_empty0);
+    const bool need_mask = (j * TC_BC + TC_BC > kv_len) || (p.causal && j * TC_BC + TC_BC - 1 > q0);
+    if (need_mask) {
+#pragma unroll
+      for (int t = 0; t < 64; ++t) {
+        const int col = j * TC_BC + (t >> 2) * 8 + q2 + (t & 1);
+        const int row = rows[(t >> 1) & 1];
+        if (!((col < kv_len) && (!p.causal || col <= row))) sacc[t] = -INFINITY;
+      }
+    }
+    float f[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int t = 0; t < 16; ++t) mx = fmaxf(mx, fmaxf(sacc[4 * t + 2 * i], sacc[4 * t + 2 * i + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[i], mx * sl2);
+      f[i] = (m_new == -INFINITY) ? 1.f : fast_exp2(m_run[i] - m_new);
+      m_run[i] = m_new;
+      l_part[i] *= f[i];
+      const float m_eff = (m_new == -INFINITY) ? 0.f : m_new;
+#pragma unroll
+      for (int t = 0; t < 16; ++t) {
+        const float e0 = fast_exp2(fmaf(sacc[4 * t + 2 * i], sl2, -m_eff));   // masked: exp2(-inf) = 0
+        const float e1 = fast_exp2(fmaf(sacc[4 * t + 2 * i + 1], sl2, -m_eff));
+        l_part[i] += e0 + e1;
+        sacc[4 * t + 2 * i] = e0;
+        sacc[4 * t + 2 * i + 1] = e1;
+      }
+    }
+    if (j > 0) {
+#pragma unroll
+      for (int t = 0; t < 64; ++t) o[t] *= f[(t >> 1) & 1];
+    }
+    uint32_t pa[TC_BC / 16][4];
+#pragma unroll
+    for (int k = 0; k < TC_BC / 16; ++k) acc_to_a(sacc, k, pa[k]);
+    mbar_wait(bf ? v_full1 : v_full0, ph);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < TC_BC / 16; ++k) wgmma_m64n128_rs<1>(o, pa[k], desc_mnmajor(sV[bf], k), (j | k) != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    consumer_release(bf ? v_empty1 : v_empty0);
+  }
+  // epilogue: combine the quad's partial row sums, normalise, store
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float l = l_part[i];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = (n_tiles > 0 && l > 0.f) ? 1.f / l : 0.f;
+    const int row = rows[i];
+    if (row < row_limit) {
+      bf16* orow = p.o + (long long)(tok0 + row) * p.ldo + (long long)h * TC_D + q2;
+#pragma unroll
+      for (int t = 0; t < 16; ++t) {
+        const float x0 = n_tiles > 0 ? o[4 * t + 2 * i] * inv : 0.f, x1 = n_tiles > 0 ? o[4 * t + 2 * i + 1] * inv : 0.f;
+        *reinterpret_cast<uint32_t*>(orow + 8 * t) = pack_bf16x2(x0, x1);
+      }
+      if ((lane & 3) == 0 && p.lse != nullptr)
+        p.lse[((long long)b * p.Hq + h) * p.T + row] = l > 0.f ? (m_run[i] + log2f(l)) / kLog2e : -INFINITY;
+    }
   }
 }
 
@@ -289,12 +224,13 @@ int mm_attn_make_tmap_stats(CUtensorMap* tm, const float* base, long long width,
   return MM_OK;
 }
 
-int mm_attn_make_tmap_rows(CUtensorMap* tm, const void* base, long long width, long long rows, long long ld) {
+int mm_attn_make_tmap_rows(CUtensorMap* tm, const void* base, long long width, long long rows, long long ld,
+                           int box_rows) {
   PFN_encodeTiled enc = tmap_encoder();
   if (!enc) return MM_ERR_CUDA;
   cuuint64_t dims[2] = {(cuuint64_t)width, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {64, 128};
+  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -330,17 +266,17 @@ int launch_fwd_tc(const void* q, const void* k, const void* v, void* o, float* l
   static std::once_flag once;
   static cudaError_t err = cudaSuccess;
   std::call_once(once, [&] {
-    err = cudaFuncSetAttribute(flash_fwd_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC2_SMEM);
+    err = cudaFuncSetAttribute(flash_fwd_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM);
   });
   MM_CHECK_CUDA(err);
-  flash_fwd_tc2_kernel<<<grid, TC2_THREADS, TC2_SMEM, stream>>>(tq, tk, tv, p);
+  flash_fwd_wgmma_kernel<<<grid, TC_THREADS, TC_SMEM, stream>>>(tq, tk, tv, p);
   MM_CHECK_LAUNCH();
   return MM_OK;
 }
 
 }  // namespace
 
-// tcgen05 flash-attention forward, head_dim 128. Same argument meaning as mm_attn_fwd.
+// wgmma flash-attention forward, head_dim 128. Same argument meaning as mm_attn_fwd.
 MM_API int mm_attn_fwd_tc(const void* q, const void* k, const void* v, void* o, float* lse,
                           const int* seqlens, long long ldq, long long ldk, long long ldv, long long ldo,
                           int B, int T, int Hq, int Hkv, int head_dim, int causal, float scale,

@@ -1,83 +1,43 @@
-// metamorph_b200 — helpers shared by the tcgen05 attention kernels (attention_tc.cu forward, attention_bwd_tc.cu
-// backward): TS-form MMA, TMEM stores, SW128 operand descriptors for the [128 x 64] TMA boxes, row tensor maps.
+// metamorph_b200 — helpers shared by the wgmma attention kernels (attention_tc.cu forward, attention_bwd_tc.cu
+// backward): SW128 operand descriptors for the [128 x 64] TMA boxes, accumulator -> A-fragment packing, row tensor maps.
 #pragma once
-#include "common.cuh"
+#include "wgmma.cuh"
 #include <mutex>
 
 namespace mm_attn_tc {
 
 constexpr float kLog2e = 1.4426950408889634f;
 
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-      "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-      "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-      "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(r[0]),
-               "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
 
-// K-major SW128 operand tile stored as two [128 rows x 64 elem] TMA boxes (16 KB each)
+// K-major SW128 operand tile stored as two [rows x 64 elem] TMA boxes of 128 rows (16 KB each): k16-th 16-wide slice
 __device__ __forceinline__ uint64_t desc_kmajor(uint32_t tile, int k16) {
-  const uint32_t addr = tile + (uint32_t)(k16 >> 2) * 16384u + (uint32_t)(k16 & 3) * 32u;
-  return (uint64_t)((addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) |
-         (2ull << 61);
+  return wgmma_desc(tile + (uint32_t)(k16 >> 2) * 16384u + (uint32_t)(k16 & 3) * 32u, 16);
 }
 // MN-major SW128 operand tile: two [128 k-rows x 64 mn-elem] boxes; LBO = 16 KB between MN chunks
 __device__ __forceinline__ uint64_t desc_mnmajor(uint32_t tile, int k16) {
-  const uint32_t addr = tile + (uint32_t)k16 * 2048u;
-  return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)(16384 >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) |
-         (1ull << 46) | (2ull << 61);
+  return wgmma_desc(tile + (uint32_t)k16 * 2048u, 16384);
 }
-
+// fp32 accumulator columns [16k, 16k + 16) of a wgmma D fragment -> the bf16 A fragment of k-slice k
+template <int NA>
+__device__ __forceinline__ void acc_to_a(const float (&d)[NA], int k, uint32_t (&a)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) a[i] = pack_bf16x2(d[8 * k + 2 * i], d[8 * k + 2 * i + 1]);
+}
+// Release a shared-memory stage: one arrive per warp of the consumer warpgroups (barrier count 8).
+__device__ __forceinline__ void consumer_release(uint32_t bar) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
+}
 
 }  // namespace mm_attn_tc
 
-// One tensor map per operand: rows = tokens, box = [128 rows x 64 bf16] (128-byte swizzle). Defined in attention_tc.cu.
-int mm_attn_make_tmap_rows(CUtensorMap* tm, const void* base, long long width, long long rows, long long ld);
+// One tensor map per operand: rows = tokens, box = [box_rows x 64 bf16] (128-byte swizzle). Defined in attention_tc.cu.
+int mm_attn_make_tmap_rows(CUtensorMap* tm, const void* base, long long width, long long rows, long long ld,
+                           int box_rows = 128);
 // fp32 statistics rows [rows, width] (lse*log2e and delta of the backward): box = 128 values of one row.
 int mm_attn_make_tmap_stats(CUtensorMap* tm, const float* base, long long width, long long rows);

@@ -1,6 +1,6 @@
-// metamorph_b200 — shared device/host helpers for the sm_100a kernels.
-// Everything here is hand-written for Blackwell (B200): mbarrier, TMA, tcgen05 PTX wrappers,
-// warp-shuffle reductions, 128-bit global access helpers and the C-ABI error plumbing.
+// metamorph_b200 — shared device/host helpers for the sm_90a kernels.
+// Hand-written for Hopper (H100): mbarrier, TMA, cp.async / ldmatrix / mma.sync PTX wrappers,
+// warp-shuffle reductions, 128-bit global access helpers and the C-ABI error plumbing (wgmma lives in wgmma.cuh).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -47,13 +47,16 @@ void mm_set_error(const char* fmt, ...);
 static inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
 int mm_num_sms();
+// Zero-initialised device scratch private to (current device, stream, tag), grown on demand. Kernels that use it leave
+// it as they found it (or overwrite it fully), so stream-ordered calls can reuse it; calls on different streams never
+// share it. nullptr (with the error text set) when the allocation fails.
+void* mm_stream_scratch(int tag, size_t bytes, cudaStream_t stream);
+enum { MM_SCRATCH_LOSS = 0, MM_SCRATCH_RMSNORM_DW = 1 };
 // programmatic dependent launch (PDL) for the decode chain: 1 unless MM_PDL=0 (api.cu)
 int mm_pdl_enabled();
 // MM_PDL_MODE bitmask (default 3): 1 = weight-streaming GEMMs launched with the PDL attribute, 2 = the small decode kernels
-// too, 8 = trigger dependents after the main loop instead of at kernel entry. B200 sweep of the 512-step batch-8 decode with
-// the round-2 TMA kernel (activations travel with the weight stage): off 3.836 ms/step, 1: 3.617, 3: 3.609, 9: 3.694,
-// 11: 3.678 — the early trigger lets the next kernel's producer fill its ring with weights while this one drains
-// (round 1's register-staged kernels preferred the late trigger, mode 9).
+// too, 8 = trigger dependents after the main loop instead of at kernel entry. The early trigger lets the next kernel's
+// producer fill its ring with weights while this one drains.
 int mm_pdl_mode();
 
 // ----------------------------------------------------------------------------------------------
@@ -200,18 +203,15 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug becomes a trap (launch failure) instead of a hung GPU box. The bound is in TIME (about
+// Bounded wait: a protocol bug becomes a trap (launch failure) instead of a hung GPU. The bound is in TIME (about
 // two seconds of SM clock): one try_wait may itself block for a hardware-defined interval, so a spin count says little.
+// No printf here: a call in a kernel that issues wgmma makes ptxas serialise every wgmma of the kernel.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 0x3FFu) == 0 && clock64() - t0 > 4000000000ll) {
-      printf("mbar_wait timeout: block (%d,%d,%d) thread %d bar %u parity %u\n", (int)blockIdx.x, (int)blockIdx.y,
-             (int)blockIdx.z, (int)threadIdx.x, bar, parity);
-      __trap();
-    }
+    if ((++spins & 0x3FFu) == 0 && clock64() - t0 > 4000000000ll) __trap();
   }
 }
 
@@ -228,62 +228,6 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const void* tmap,
       ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c_inner),
       "r"(c_outer)
       : "memory");
-}
-
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tcgen05_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_result_addr) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_result_addr),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; bf16 inputs, fp32 accumulate.
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all tcgen05 ops previously issued by this thread have completed.
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   bar)
-               : "memory");
-}
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 
 // ---------------------------------------------------------------- cp.async / ldmatrix / mma.sync

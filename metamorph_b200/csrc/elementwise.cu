@@ -82,20 +82,30 @@ __global__ void gelu_bwd_kernel(const bf16* __restrict__ z, const bf16* __restri
   }
 }
 
-// out[n] (+)= sum_r x[r, n]; one thread per column pair, rows strided over blockIdx.y
-__global__ void colsum_kernel(const bf16* __restrict__ x, float* __restrict__ out, long long R,
-                              long long N, long long ld) {
-  const long long col = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 2;
-  if (col >= N) return;
+// out[n] (+)= sum_r x[r, n]. One block owns 64 columns (32 column pairs x 8 row phases); each thread adds its rows in
+// order and the 8 phases are combined in order, so the sum does not depend on scheduling (bias gradients are the same
+// bits on every run).
+__global__ void __launch_bounds__(256) colsum_kernel(const bf16* __restrict__ x, float* __restrict__ out, long long R,
+                                                     long long N, long long ld) {
+  __shared__ float2 part[8][32];
+  const long long col = ((long long)blockIdx.x * 32 + threadIdx.x) * 2;
   float s0 = 0.f, s1 = 0.f;
-  for (long long r = blockIdx.y; r < R; r += gridDim.y) {
-    const bf162 v = *reinterpret_cast<const bf162*>(x + r * ld + col);
-    const float2 f = __bfloat1622float2(v);
-    s0 += f.x;
-    s1 += f.y;
+  if (col < N) {
+    for (long long r = threadIdx.y; r < R; r += 8) {
+      const float2 f = __bfloat1622float2(*reinterpret_cast<const bf162*>(x + r * ld + col));
+      s0 += f.x;
+      s1 += f.y;
+    }
   }
-  atomicAdd(out + col, s0);
-  if (col + 1 < N) atomicAdd(out + col + 1, s1);
+  part[threadIdx.y][threadIdx.x] = make_float2(s0, s1);
+  __syncthreads();
+  if (threadIdx.y != 0 || col >= N) return;
+  for (int k = 1; k < 8; ++k) {
+    s0 += part[k][threadIdx.x].x;
+    s1 += part[k][threadIdx.x].y;
+  }
+  out[col] += s0;
+  if (col + 1 < N) out[col + 1] += s1;
 }
 
 // images [N,3,S,S] (bf16, NCHW) -> patches [N*(S/14)^2, ldp]; column = c*196 + ky*14 + kx
@@ -197,8 +207,7 @@ MM_API int mm_gelu_bwd(const void* z, const void* da, void* dz, long long n, cud
 MM_API int mm_colsum_accum(const void* x, float* out, long long R, long long N, long long ld,
                            cudaStream_t stream) {
   MM_CHECK_ARG(R > 0 && N > 0 && N % 2 == 0 && ld % 2 == 0, "mm_colsum_accum: N, ld must be even");
-  dim3 grid((unsigned)ceil_div64(N / 2, 128), (unsigned)(R < 64 ? R : 64));
-  colsum_kernel<<<grid, 128, 0, stream>>>((const bf16*)x, out, R, N, ld);
+  colsum_kernel<<<(unsigned)ceil_div64(N, 64), dim3(32, 8), 0, stream>>>((const bf16*)x, out, R, N, ld);
   MM_CHECK_LAUNCH();
   return MM_OK;
 }

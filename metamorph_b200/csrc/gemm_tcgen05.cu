@@ -1,5 +1,6 @@
-// metamorph_b200 — bf16 GEMM on 5th-gen tensor cores (tcgen05.mma, accumulators in TMEM, operands
+// metamorph_b200 — bf16 GEMM on Hopper tensor cores (wgmma.mma_async, fp32 accumulators in registers, operands
 // staged by TMA into 128B-swizzled shared memory), persistent + warp-specialised, fused epilogues.
+// (This file keeps its historical name; nothing in it uses tcgen05.)
 //
 // One kernel family serves every dense contraction on the hot path (SURVEY.md §2.1 K1,K3,K5,K6,K8,
 // K11,K13,K14,K15,K16 and their dgrad/wgrad):
@@ -7,15 +8,15 @@
 //     C[M,N] = A[M,K] * B[K,N]             (dgrad  dX = dY * W;  A K-major,  B MN-major)
 //     C[M,N] = A[K,M]^T * B[K,N]           (wgrad  dW = dY^T X;  A MN-major, B MN-major)
 // "K-major" = the contraction index is the contiguous one in memory. MN-major operands are fed to
-// the tensor core directly through the UMMA shared-memory descriptor (no transpose pass).
+// the tensor core directly through the wgmma transpose bits of the shared-memory descriptors (no transpose pass).
 //
-// CTA layout (256 threads, 1 CTA/SM, grid = min(#tiles, #SMs), static persistent schedule):
-//   warp 0 lane 0 : TMA producer        (global -> smem ring, kStages deep, mbarrier tx-count)
-//   warp 1 lane 0 : MMA issuer          (tcgen05.mma 128 x BN x 16, commit -> frees smem stage)
-//   warp 2        : TMEM allocator      (2 accumulator stages x BN fp32 columns)
-//   warps 4..7    : epilogue            (tcgen05.ld 32x32b -> registers -> fused math -> global)
-// The accumulator is double-buffered in TMEM so the epilogue of tile i overlaps the MMAs of i+1.
-#include "common.cuh"
+// CTA layout (384 threads, 1 CTA/SM, grid = min(#tiles, #SMs), static persistent schedule, tile BM=128 x BN):
+//   warpgroup 0, one thread : TMA producer (global -> smem ring, kStages deep, mbarrier tx-count); it keeps loading
+//                             the next tile while the consumers run the epilogue of the current one
+//   warpgroups 1, 2         : consumers, 64 rows each: wgmma m64nBNk16 per 16-wide k-slice, then the fused epilogue
+//                             (accumulators -> padded smem staging, 64 columns at a time -> one row x 32 columns per
+//                             thread -> epilogue_chunk -> global)
+#include "wgmma.cuh"
 #include <mutex>
 #include <stdlib.h>
 
@@ -23,8 +24,8 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BK = 64;       // 64 bf16 = 128 bytes = one swizzle-128B row
-constexpr int UMMA_K = 16;
-constexpr int kThreads = 256;
+constexpr int kThreads = 384;
+constexpr int kStageLd = 68;  // fp32 pitch of the epilogue staging rows (64 + 4: conflict-free float4 row reads)
 
 enum Epilogue : int {
   EPI_STORE = 0,           // C = acc
@@ -50,48 +51,18 @@ struct EpiParams {
   int out_f32;     // 1: C is fp32, 0: bf16
   int accumulate;  // 1: C += result (C read in its own dtype)
   float alpha;     // result scale applied to acc before everything else
-  int tma_store;   // 1: bf16 result leaves through shared memory + cp.async.bulk.tensor stores (2-CTA kernel)
 };
 
 template <int BN>
 struct Cfg {
-  static constexpr int kStages = (BN == 256) ? 4 : 6;
+  static constexpr int kStages = (BN == 256) ? 3 : 5;
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kTmemCols = 2 * BN;  // two accumulator stages
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int kEpiBytes = 2 * 64 * kStageLd * 4;   // one [64 x 64] fp32 staging tile per consumer warpgroup
+  static constexpr int kSmemBytes = kStages * kStageBytes + kEpiBytes + 1024 /*align*/ + 256 /*barriers*/;
+  static_assert(kSmemBytes <= 227 * 1024, "shared memory budget of one H100 CTA");
 };
-
-__device__ __forceinline__ uint64_t make_desc_base(bool mn_major) {
-  // Shared-memory matrix descriptor (tcgen05): start[0,14) | LBO[16,30) | SBO[32,46) |
-  // version=1 [46,48) | layout_type[61,64) (2 = SWIZZLE_128B). Offsets are in 16-byte units.
-  const uint64_t sbo = 1024 >> 4;                           // 8 rows x 128 B
-  const uint64_t lbo = mn_major ? ((BK * 128) >> 4) : 1;    // MN-major: next 64-element MN chunk
-  return (lbo << 16) | (sbo << 32) | (1ull << 46) | (2ull << 61);
-}
-
-// L2 eviction-priority hints for the operand streams (TMA .L2::cache_hint). Within one rasterisation group the A panel
-// (group_m row-blocks x K) is re-read by every column-block of the sweep -> keep it (evict_last); a B column-block is
-// consumed by the concurrently running tiles of one wave and not touched again before the next group -> evict_first.
-__device__ __forceinline__ uint64_t l2_policy_evict_last() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
-__device__ __forceinline__ void tma_load_2d_hint(uint32_t smem_dst, const void* tmap, uint32_t bar, int32_t c_inner,
-                                                 int32_t c_outer, uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_dst),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c_inner), "r"(c_outer), "l"(policy)
-      : "memory");
-}
 
 // Fused epilogue for one 32-column accumulator chunk held by one thread (one output row).
 __device__ __forceinline__ void epilogue_chunk(const EpiParams& ep, float (&v)[32], int row, bool row_ok,
@@ -180,7 +151,7 @@ __device__ __forceinline__ void epilogue_chunk(const EpiParams& ep, float (&v)[3
 #pragma unroll
       for (int j = 0; j < 32; ++j) v[j] = gelu_tanh(v[j]);
     }
-    if (!row_ok) return;  // lanes past M only take part in the TMEM load
+    if (!row_ok) return;
     if (ep.epi == EPI_RESID || ep.epi == EPI_BIAS_RESID) {
       const bf16* rp = ep.resid + (long long)row * ep.ldr + col0;
       if (full_chunk) {
@@ -244,100 +215,41 @@ __device__ __forceinline__ void epilogue_chunk(const EpiParams& ep, float (&v)[3
       }
     }
 }
-// The store-free part of the plain epilogues (STORE / BIAS / BIAS_GELU_* / RESID / BIAS_RESID, bf16 out, no accumulate):
-// v -> bias -> activation -> residual, packed to 16 bf16x2 words (the TMA-store path writes them to shared memory).
-__device__ __forceinline__ void epilogue_pack_chunk(const EpiParams& ep, float (&v)[32], int row, bool row_ok, int col0,
-                                                    int N, uint32_t (&out)[16]) {
-  const bool full_chunk = (col0 + 32 <= N);
-  if (ep.epi == EPI_BIAS || ep.epi == EPI_BIAS_GELU_ERF || ep.epi == EPI_BIAS_GELU_TANH || ep.epi == EPI_BIAS_RESID) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j)
-      if (full_chunk || col0 + j < N) v[j] += __bfloat162float(__ldg(ep.bias + col0 + j));
-  }
-  if (ep.epi == EPI_BIAS_GELU_ERF) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
-  } else if (ep.epi == EPI_BIAS_GELU_TANH) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = gelu_tanh(v[j]);
-  }
-  if (row_ok && (ep.epi == EPI_RESID || ep.epi == EPI_BIAS_RESID)) {
-    const bf16* rp = ep.resid + (long long)row * ep.ldr + col0;
-    if (full_chunk) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 8) {
-        const int4 rr = *reinterpret_cast<const int4*>(rp + j);
-        float2 f;
-        f = unpack_bf16x2(rr.x); v[j] += f.x; v[j + 1] += f.y;
-        f = unpack_bf16x2(rr.y); v[j + 2] += f.x; v[j + 3] += f.y;
-        f = unpack_bf16x2(rr.z); v[j + 4] += f.x; v[j + 5] += f.y;
-        f = unpack_bf16x2(rr.w); v[j + 6] += f.x; v[j + 7] += f.y;
-      }
-    } else {
-      for (int j = 0; j < 32; ++j)
-        if (col0 + j < N) v[j] += __bfloat162float(rp[j]);
-    }
-  }
-#pragma unroll
-  for (int j = 0; j < 16; ++j) out[j] = pack_bf16x2(v[2 * j], v[2 * j + 1]);
-}
 
-// 2-D tiled store shared -> global (the tensor map clips rows / columns past the matrix)
-__device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t smem_src, int32_t c_inner, int32_t c_outer) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(tmap)),
-               "r"(smem_src), "r"(c_inner), "r"(c_outer)
-               : "memory");
+// D[64 x BN] (+)= A * B for one 16-wide k-slice; the transpose bits are template arguments of the instruction
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void wgmma_k16(float (&d)[BN / 2], uint64_t da, uint64_t db, uint32_t acc) {
+  if constexpr (BN == 256) wgmma_m64n256_ss<TA, TB>(d, da, db, acc);
+  else wgmma_m64n128_ss<TA, TB>(d, da, db, acc);
 }
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 template <int BN, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(kThreads, 1)
-gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                    const __grid_constant__ CUtensorMap tmap_b, int M, int N, int K, int group_m,
-                    EpiParams ep) {
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, int M, int N,
+                  int K, int group_m, EpiParams ep) {
   using C = Cfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + C::kStages * C::kStageBytes;
+  const uint32_t epi_base = smem_base + C::kStages * C::kStageBytes;
+  const uint32_t bar_base = epi_base + C::kEpiBytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (C::kStages + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * C::kStages + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * C::kStages + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * C::kStages + 4);
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int num_m = (M + BM - 1) / BM, num_n = (N + BN - 1) / BN;
   const int num_tiles = num_m * num_n;
   const int num_kb = (K + BK - 1) / BK;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < C::kStages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), 4);  // one arrive per epilogue warp
+      mbar_init(empty_bar(s), 8);   // one arrive per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc<C::kTmemCols>(tmem_slot);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
   auto tile_coords = [&](int t, int& m_blk, int& n_blk) {
     // rasterisation: a group of `group_m` row-blocks (its A panel sized to stay L2-resident) sweeps all
@@ -351,505 +263,101 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a,
     n_blk = r / gsz;
   };
 
-  if (warp == 0 && lane == 0) {
+  if (wg == 0) {
     // ------------------------------------------------------------------ TMA producer
-    int s = 0;
-    uint32_t phase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      int m_blk, n_blk;
-      tile_coords(t, m_blk, n_blk);
-      const int m0 = m_blk * BM, n0 = n_blk * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(empty_bar(s), phase ^ 1);
-        const uint32_t sa = smem_base + s * C::kStageBytes;
-        const uint32_t sb = sa + C::kABytes;
-        mbar_arrive_expect_tx(full_bar(s), C::kStageBytes);
-        const int k0 = kb * BK;
-        if constexpr (!A_MN) {
-          tma_load_2d(sa, &tmap_a, full_bar(s), k0, m0);
-        } else {
-#pragma unroll
-          for (int j = 0; j < BM / 64; ++j)
-            tma_load_2d(sa + j * (BK * 128), &tmap_a, full_bar(s), m0 + 64 * j, k0);
-        }
-        if constexpr (!B_MN) {
-          tma_load_2d(sb, &tmap_b, full_bar(s), k0, n0);
-        } else {
-#pragma unroll
-          for (int j = 0; j < BN / 64; ++j)
-            tma_load_2d(sb + j * (BK * 128), &tmap_b, full_bar(s), n0 + 64 * j, k0);
-        }
-        if (++s == C::kStages) { s = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1 && lane == 0) {
-    // ------------------------------------------------------------------ MMA issuer
-    // Instruction descriptor (kind::f16): D=f32 [4,6)=1, A=bf16 [7,10)=1, B=bf16 [10,13)=1,
-    // a_major bit15, b_major bit16 (1 = MN-major), N>>3 at [17,23), M>>4 at [24,29).
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (uint32_t(A_MN) << 15) |
-                           (uint32_t(B_MN) << 16) | (uint32_t(BN >> 3) << 17) |
-                           (uint32_t(BM >> 4) << 24);
-    const uint64_t desc_a_base = make_desc_base(A_MN);
-    const uint64_t desc_b_base = make_desc_base(B_MN);
-    // bytes to advance the operand start address per UMMA_K (=16) step
-    constexpr uint32_t a_kstep = A_MN ? (UMMA_K * 128) : (UMMA_K * 2);
-    constexpr uint32_t b_kstep = B_MN ? (UMMA_K * 128) : (UMMA_K * 2);
-    int s = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      mbar_wait(tempty_bar(acc), acc_phase ^ 1);
-      tcgen05_fence_after();
-      const uint32_t tmem_d = tmem_base + acc * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(full_bar(s), phase);
-        tcgen05_fence_after();
-        const uint32_t sa = smem_base + s * C::kStageBytes;
-        const uint32_t sb = sa + C::kABytes;
-#pragma unroll
-        for (int k = 0; k < BK / UMMA_K; ++k) {
-          const uint64_t da = desc_a_base | uint64_t(((sa + k * a_kstep) & 0x3FFFFu) >> 4);
-          const uint64_t db = desc_b_base | uint64_t(((sb + k * b_kstep) & 0x3FFFFu) >> 4);
-          umma_bf16_ss(tmem_d, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-        }
-        umma_commit(empty_bar(s));                          // smem stage reusable once MMAs retire
-        if (kb == num_kb - 1) umma_commit(tfull_bar(acc));  // accumulator ready for the epilogue
-        if (++s == C::kStages) { s = 0; phase ^= 1; }
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------------ epilogue warps
-    const int q = warp & 3;  // TMEM lane quadrant this warp may access
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      int m_blk, n_blk;
-      tile_coords(t, m_blk, n_blk);
-      const int row = m_blk * BM + q * 32 + lane;
-      const int n0 = n_blk * BN;
-      const bool row_ok = row < M;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tcgen05_fence_after();
-      const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16) + acc * BN;
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        const int col0 = n0 + c * 32;
-        if (col0 >= N) break;  // warp-uniform
-        __syncwarp();          // reconverge before the .aligned TMEM load
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(taddr + c * 32, r);
-        tmem_ld_wait();
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) * ep.alpha;
-        epilogue_chunk(ep, v, row, row_ok, col0, N);
-      }
-      // all TMEM reads of this accumulator stage are complete (tcgen05.wait::ld above)
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  }
-
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tcgen05_fence_after();
-    tmem_dealloc<C::kTmemCols>(tmem_base);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// 2-CTA variant (tcgen05 cta_group::2): a cluster of two CTAs on one TPC computes a 256 x 256 output tile.
-// Each CTA stages ITS 128 rows of A and ITS half (128 of 256 columns) of B; the leader CTA issues
-// tcgen05.mma.cta_group::2 (M=256) which reads B from both CTAs' shared memory, so every B byte is
-// loaded from L2 and read from smem once per pair instead of once per CTA (33 % less operand traffic per
-// flop: the train step is power-capped, energy per flop is what buys clocks). Accumulator rows live in
-// the TMEM of the CTA that owns them; barriers are per CTA at identical smem offsets:
-//   full[s]   (leader's)  count 2: leader arrive.expect_tx(both CTAs' bytes) + peer's remote arrive;
-//                         both CTAs' TMA loads complete_tx on the leader's barrier (peer bit masked)
-//   empty[s], tfull[a]    signalled in BOTH CTAs by the leader's multicast tcgen05.commit
-//   tempty[a] (leader's)  count 8: the four epilogue warps of both CTAs (peer warps arrive remotely)
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t bar, uint32_t cta) {
-  asm volatile(
-      "{\n"
-      ".reg .b32 ra;\n"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n"
-      "}\n" ::"r"(bar),
-      "r"(cta)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t smem_dst, const void* tmap, uint32_t bar,
-                                                int32_t c_inner, int32_t c_outer) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_dst),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar & 0xFEFFFFFFu), "r"(c_inner), "r"(c_outer)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm_hint(uint32_t smem_dst, const void* tmap, uint32_t bar,
-                                                     int32_t c_inner, int32_t c_outer, uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_dst),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar & 0xFEFFFFFFu), "r"(c_inner), "r"(c_outer), "l"(policy)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_ss_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                                 uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          bar),
-      "h"((uint16_t)3)
-      : "memory");
-}
-
-// ---- cluster launch control (Blackwell work stealing): a running cluster atomically cancels a cluster of the SAME grid
-// that has not been launched yet and computes its tile. The 16-byte response lands (multicast) at the same shared-memory
-// offset of every CTA of the cluster and completes 16 tx-bytes on each CTA's mbarrier at the same offset.
-__device__ __forceinline__ void clc_try_cancel_multicast(uint32_t resp, uint32_t bar) {
-  asm volatile(
-      "clusterlaunchcontrol.try_cancel.async.shared::cta.mbarrier::complete_tx::bytes.multicast::cluster::all.b128 "
-      "[%0], [%1];" ::"r"(resp), "r"(bar)
-      : "memory");
-}
-// -> first CTA index (x) of the cancelled cluster, or -1 when nothing was left to cancel
-__device__ __forceinline__ int clc_response_ctaid_x(uint32_t resp) {
-  uint32_t x, ok;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      ".reg .b128 r;\n"
-      "ld.shared.b128 r, [%2];\n"
-      "clusterlaunchcontrol.query_cancel.is_canceled.pred.b128 p, r;\n"
-      "selp.u32 %1, 1, 0, p;\n"
-      "mov.u32 %0, 0;\n"
-      "@p clusterlaunchcontrol.query_cancel.get_first_ctaid.v4.b32.b128 {%0, _, _, _}, r;\n"
-      "}\n"
-      : "=r"(x), "=r"(ok)
-      : "r"(resp)
-      : "memory");
-  return ok ? (int)x : -1;
-}
-
-constexpr int BN2 = 256;             // cluster tile N
-constexpr int kClcStages = 3;        // tile-id responses in flight / not yet read by the slowest role
-constexpr int kStages2 = 6;
-constexpr int kA2Bytes = BM * BK * 2;          // this CTA's 128 rows of A
-constexpr int kB2Bytes = (BN2 / 2) * BK * 2;   // this CTA's 128 columns of B
-constexpr int kStage2Bytes = kA2Bytes + kB2Bytes;
-constexpr int kCStageBytes = 128 * 64 * 2;   // one [128 rows x 64 cols] bf16 staging tile of the TMA-store epilogue
-constexpr int kSmem2Bytes = kStages2 * kStage2Bytes + 2 * kCStageBytes + 1024 + 384;   // + alignment slack + barriers / CLC responses
-
-// Tile schedule. DYN = false: static persistent (cluster c computes tiles c, c + #clusters, ...). DYN = true (default):
-// the grid holds ONE cluster per tile and every resident cluster keeps stealing not-yet-launched clusters through
-// cluster launch control, so an SM pair that starts late or runs slow — it shares its SMs / HBM with the NCCL channels
-// and the AdamW of the previous layer's gradient bucket — simply computes fewer tiles instead of holding up its wave.
-template <bool A_MN, bool B_MN, bool DYN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
-gemm_tcgen05_2cta_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                         const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_c,
-                         int M, int N, int K, int group_m, int l2_hint, EpiParams ep) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t cstage_base = smem_base + kStages2 * kStage2Bytes;      // 1024-aligned: 128-byte swizzle atoms
-  const uint32_t bar_base = cstage_base + 2 * kCStageBytes;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (kStages2 + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * kStages2 + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * kStages2 + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * kStages2 + 4);
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-  auto clc_full = [&](int c) { return bar_base + 8u * (2 * kStages2 + 5 + c); };
-  auto clc_empty = [&](int c) { return bar_base + 8u * (2 * kStages2 + 5 + kClcStages + c); };
-  auto clc_resp = [&](int c) { return bar_base + 8u * (2 * kStages2 + 6 + 2 * kClcStages) + 16u * c; };   // 16-byte aligned
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int num_m = (M + 2 * BM - 1) / (2 * BM), num_n = (N + BN2 - 1) / BN2;
-  const int num_tiles = num_m * num_n;
-  const int num_kb = (K + BK - 1) / BK;
-  const int cluster_id = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmap_a);
-    prefetch_tmap(&tmap_b);
-    if (ep.tma_store) prefetch_tmap(&tmap_c);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kStages2; ++s) {
-      mbar_init(full_bar(s), 2);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), 8);
-    }
-    for (int c = 0; c < kClcStages; ++c) {
-      mbar_init(clc_full(c), 1);     // this CTA's producer arms it (arrive.expect_tx 16), the response completes it
-      mbar_init(clc_empty(c), 11);   // (leader's only) producer + MMA + 4 epilogue warps here, producer + 4 warps in the peer
-    }
-    fence_barrier_init();
-  }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "n"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
-  cluster_sync_all();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-
-  auto tile_coords = [&](int t, int& m_blk, int& n_blk) {
-    const int per_group = group_m * num_n;
-    const int g = t / per_group;
-    const int first_m = g * group_m;
-    const int gsz = min(group_m, num_m - first_m);
-    const int r = t - g * per_group;
-    m_blk = first_m + (r % gsz);
-    n_blk = r / gsz;
-  };
-  // Every role walks the same tile sequence. Static: t += #clusters. Dynamic: the producer thread of each CTA arms
-  // clc_full[c] before it starts a tile and the leader's producer issues the steal; every role then reads the response
-  // when it is done with its part of the current tile and releases the slot on the LEADER's clc_empty[c].
-  auto next_tile = [&](int t, int& c, uint32_t& cph, bool one_thread) -> int {
-    if constexpr (!DYN) {
-      t += num_clusters;
-      return t < num_tiles ? t : -1;
-    } else {
-      mbar_wait(clc_full(c), cph);
-      const int x = clc_response_ctaid_x(clc_resp(c));
-      fence_proxy_async_smem();                  // the slot is rewritten by the async proxy
-      if (!one_thread) __syncwarp();
-      if (one_thread || lane == 0) {
-        if (leader) mbar_arrive(clc_empty(c));
-        else mbar_arrive_remote(clc_empty(c), 0);
-      }
-      if (++c == kClcStages) { c = 0; cph ^= 1; }
-      return x < 0 ? -1 : (x >> 1);
-    }
-  };
-
-  if (warp == 0 && lane == 0) {
-    // ------------------------------------------------------------------ TMA producer (both CTAs)
-    int s = 0;
-    uint32_t phase = 0;
-    const uint64_t pol_a = l2_policy_evict_last(), pol_b = l2_policy_evict_first();
-    int cq = 0, cc = 0;                 // response slot being requested / consumed
-    uint32_t cqph = 0, ccph = 0;
-    for (int t = cluster_id; t >= 0 && t < num_tiles;) {
-      if constexpr (DYN) {              // ask for the NEXT tile before streaming this one
-        if (leader) mbar_wait(clc_empty(cq), cqph ^ 1);     // every role of both CTAs has read the slot's previous use
-        mbar_arrive_expect_tx(clc_full(cq), 16);
-        if (leader) clc_try_cancel_multicast(clc_resp(cq), clc_full(cq));
-        if (++cq == kClcStages) { cq = 0; cqph ^= 1; }
-      }
-      int m_blk, n_blk;
-      tile_coords(t, m_blk, n_blk);
-      const int m0 = m_blk * 2 * BM + (int)rank * BM;
-      const int n0 = n_blk * BN2 + (int)rank * (BN2 / 2);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(empty_bar(s), phase ^ 1);
-        const uint32_t sa = smem_base + s * kStage2Bytes;
-        const uint32_t sb = sa + kA2Bytes;
-        if (leader) mbar_arrive_expect_tx(full_bar(s), 2 * kStage2Bytes);
-        else mbar_arrive_remote(full_bar(s), 0);
-        const int k0 = kb * BK;
-        if (l2_hint) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      int s = 0;
+      uint32_t phase = 0;
+      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        int m_blk, n_blk;
+        tile_coords(t, m_blk, n_blk);
+        const int m0 = m_blk * BM, n0 = n_blk * BN;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(empty_bar(s), phase ^ 1);
+          const uint32_t sa = smem_base + s * C::kStageBytes;
+          const uint32_t sb = sa + C::kABytes;
+          mbar_arrive_expect_tx(full_bar(s), C::kStageBytes);
+          const int k0 = kb * BK;
           if constexpr (!A_MN) {
-            tma_load_2d_2sm_hint(sa, &tmap_a, full_bar(s), k0, m0, pol_a);
+            tma_load_2d(sa, &tmap_a, full_bar(s), k0, m0);
           } else {
 #pragma unroll
-            for (int j = 0; j < BM / 64; ++j)
-              tma_load_2d_2sm_hint(sa + j * (BK * 128), &tmap_a, full_bar(s), m0 + 64 * j, k0, pol_a);
+            for (int j = 0; j < BM / 64; ++j) tma_load_2d(sa + j * (BK * 128), &tmap_a, full_bar(s), m0 + 64 * j, k0);
           }
           if constexpr (!B_MN) {
-            tma_load_2d_2sm_hint(sb, &tmap_b, full_bar(s), k0, n0, pol_b);
+            tma_load_2d(sb, &tmap_b, full_bar(s), k0, n0);
           } else {
 #pragma unroll
-            for (int j = 0; j < BN2 / 2 / 64; ++j)
-              tma_load_2d_2sm_hint(sb + j * (BK * 128), &tmap_b, full_bar(s), n0 + 64 * j, k0, pol_b);
+            for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * (BK * 128), &tmap_b, full_bar(s), n0 + 64 * j, k0);
           }
-        } else {
-          if constexpr (!A_MN) {
-            tma_load_2d_2sm(sa, &tmap_a, full_bar(s), k0, m0);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BM / 64; ++j)
-              tma_load_2d_2sm(sa + j * (BK * 128), &tmap_a, full_bar(s), m0 + 64 * j, k0);
-          }
-          if constexpr (!B_MN) {
-            tma_load_2d_2sm(sb, &tmap_b, full_bar(s), k0, n0);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BN2 / 2 / 64; ++j)
-              tma_load_2d_2sm(sb + j * (BK * 128), &tmap_b, full_bar(s), n0 + 64 * j, k0);
-          }
+          if (++s == C::kStages) { s = 0; phase ^= 1; }
         }
-        if (++s == kStages2) { s = 0; phase ^= 1; }
       }
-      t = next_tile(t, cc, ccph, true);
     }
-  } else if (warp == 1 && lane == 0 && leader) {
-    // ------------------------------------------------------------------ MMA issuer (leader CTA only)
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (uint32_t(A_MN) << 15) |
-                           (uint32_t(B_MN) << 16) | (uint32_t(BN2 >> 3) << 17) |
-                           (uint32_t((2 * BM) >> 4) << 24);
-    const uint64_t desc_a_base = make_desc_base(A_MN);
-    const uint64_t desc_b_base = make_desc_base(B_MN);
-    constexpr uint32_t a_kstep = A_MN ? (UMMA_K * 128) : (UMMA_K * 2);
-    constexpr uint32_t b_kstep = B_MN ? (UMMA_K * 128) : (UMMA_K * 2);
+  } else {
+    // ------------------------------------------------------------------ consumers: rows [64 c, 64 c + 64) of the tile
+    setmaxnreg_inc<232>();
+    const int c = wg - 1;
+    const int tid = threadIdx.x & 127, warp_in_wg = tid >> 5;
+    // both layouts place the 64-row half c at +8 KB: K-major = 64 rows x 128 B, MN-major = the c-th 64-wide M chunk
+    constexpr uint32_t a_kstep = A_MN ? (16 * 128) : 32, b_kstep = B_MN ? (16 * 128) : 32;
+    constexpr uint32_t a_lbo = A_MN ? (BK * 128) : 16, b_lbo = B_MN ? (BK * 128) : 16;
+    float* stage = reinterpret_cast<float*>(smem_raw + (epi_base - smem_u32(smem_raw))) + c * 64 * kStageLd;
+    const int er = tid & 63, ehalf = tid >> 6;   // epilogue: this thread's row of the 64 and 32-column half of a chunk
     int s = 0;
     uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    int cc = 0;
-    uint32_t ccph = 0;
-    for (int t = cluster_id; t >= 0 && t < num_tiles; t = next_tile(t, cc, ccph, true)) {
-      mbar_wait(tempty_bar(acc), acc_phase ^ 1);
-      tcgen05_fence_after();
-      const uint32_t tmem_d = tmem_base + acc * BN2;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(full_bar(s), phase);
-        tcgen05_fence_after();
-        const uint32_t sa = smem_base + s * kStage2Bytes;
-        const uint32_t sb = sa + kA2Bytes;
-#pragma unroll
-        for (int k = 0; k < BK / UMMA_K; ++k) {
-          const uint64_t da = desc_a_base | uint64_t(((sa + k * a_kstep) & 0x3FFFFu) >> 4);
-          const uint64_t db = desc_b_base | uint64_t(((sb + k * b_kstep) & 0x3FFFFu) >> 4);
-          umma_bf16_ss_2sm(tmem_d, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-        }
-        umma_commit_2sm(empty_bar(s));
-        if (kb == num_kb - 1) umma_commit_2sm(tfull_bar(acc));
-        if (++s == kStages2) { s = 0; phase ^= 1; }
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------------ epilogue warps (both CTAs)
-    const int q = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    int cc = 0;
-    uint32_t ccph = 0;
-    for (int t = cluster_id; t >= 0 && t < num_tiles; t = next_tile(t, cc, ccph, false)) {
+    float d[BN / 2];
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
       int m_blk, n_blk;
       tile_coords(t, m_blk, n_blk);
-      const int row = m_blk * 2 * BM + (int)rank * BM + q * 32 + lane;
-      const int n0 = n_blk * BN2;
-      const bool row_ok = row < M;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tcgen05_fence_after();
-      const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16) + acc * BN2;
-      if (ep.tma_store) {
-        // TMA-store epilogue: 64 columns at a time go through a 128-byte-swizzled [128 x 64] staging tile (two of them,
-        // so the store of one overlaps the math of the next) and leave as ONE bulk tensor store per CTA — full 128-byte
-        // lines instead of 32 x 64-byte row fragments per warp; the tensor map clips the M / N tails.
-        uint8_t* cstage = smem_raw + (cstage_base - smem_u32(smem_raw));
-        const int rloc = q * 32 + lane;
-        const bool issuer = (warp == 4 && lane == 0);
-#pragma unroll 1
-        for (int pr = 0; pr < BN2 / 64; ++pr) {
-          const int colp = n0 + pr * 64;
-          if (colp >= N) break;                 // CTA-uniform
-          const int buf = pr & 1;
-          if (issuer) tma_store_wait_read<1>();  // the store issued two pairs ago has finished reading this buffer
-          asm volatile("bar.sync 1, 128;" ::: "memory");
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(full_bar(s), phase);
+        const uint32_t sa = smem_base + s * C::kStageBytes + c * (64 * 128);
+        const uint32_t sb = smem_base + s * C::kStageBytes + C::kABytes;
+        wgmma_fence();
 #pragma unroll
-          for (int h2 = 0; h2 < 2; ++h2) {
-            const int col0 = colp + h2 * 32;
-            uint32_t r[32];
-            __syncwarp();
-            tmem_ld_32x32b_x32(taddr + (pr * 2 + h2) * 32, r);
-            tmem_ld_wait();
-            float v[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) * ep.alpha;
-            uint32_t o[16];
-            if (col0 < N) {
-              epilogue_pack_chunk(ep, v, row, row_ok, col0, N, o);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) o[j] = 0u;
-            }
-            uint8_t* dst = cstage + buf * kCStageBytes + rloc * 128;
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              *reinterpret_cast<int4*>(dst + (((h2 * 4 + j) ^ (rloc & 7)) << 4)) =
-                  make_int4(o[4 * j], o[4 * j + 1], o[4 * j + 2], o[4 * j + 3]);
-          }
-          fence_proxy_async_smem();              // generic-proxy writes -> visible to the TMA engine
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-          if (issuer) {
-            tma_store_2d(&tmap_c, cstage_base + buf * kCStageBytes, colp, m_blk * 2 * BM + (int)rank * BM);
-            tma_store_commit();
-          }
-        }
-      } else {
-#pragma unroll 1
-      for (int c = 0; c < BN2 / 32; ++c) {
-        const int col0 = n0 + c * 32;
-        if (col0 >= N) break;
+        for (int k = 0; k < BK / 16; ++k)
+          wgmma_k16<BN, A_MN, B_MN>(d, wgmma_desc(sa + k * a_kstep, a_lbo), wgmma_desc(sb + k * b_kstep, b_lbo),
+                                    (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
         __syncwarp();
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(taddr + c * 32, r);
-        tmem_ld_wait();
-        float v[32];
+        if (lane == 0) mbar_arrive(empty_bar(s));   // this warp's share of the stage has been read
+        if (++s == C::kStages) { s = 0; phase ^= 1; }
+      }
+      // ---------------------------------------------------------------- epilogue, 64 columns at a time
+      const int row = m_blk * BM + c * 64 + er;
+      const bool row_ok = row < M;
+      const int g = warp_in_wg * 16 + (lane >> 2), q2 = (lane & 3) * 2;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) * ep.alpha;
-        epilogue_chunk(ep, v, row, row_ok, col0, N);
+      for (int cc = 0; cc < BN / 64; ++cc) {
+        const int colc = n_blk * BN + cc * 64;
+        if (colc >= N) break;                                 // warpgroup-uniform
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + c) : "memory");   // the previous chunk has been read
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float* src = d + 4 * (cc * 8 + j);
+          *reinterpret_cast<float2*>(stage + g * kStageLd + j * 8 + q2) = make_float2(src[0], src[1]);
+          *reinterpret_cast<float2*>(stage + (g + 8) * kStageLd + j * 8 + q2) = make_float2(src[2], src[3]);
+        }
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + c) : "memory");
+        const int col0 = colc + ehalf * 32;
+        if (col0 < N) {
+          float v[32];
+          const float* rp = stage + er * kStageLd + ehalf * 32;
+#pragma unroll
+          for (int j = 0; j < 32; j += 4) {
+            const float4 x = *reinterpret_cast<const float4*>(rp + j);
+            v[j] = x.x * ep.alpha; v[j + 1] = x.y * ep.alpha; v[j + 2] = x.z * ep.alpha; v[j + 3] = x.w * ep.alpha;
+          }
+          epilogue_chunk(ep, v, row, row_ok, col0, N);
+        }
       }
-      }
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (leader) mbar_arrive(tempty_bar(acc));
-        else mbar_arrive_remote(tempty_bar(acc), 0);
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
-  }
-
-  if (ep.tma_store && warp == 4 && lane == 0) tma_store_wait_all();   // the staging tiles must outlive their stores
-  tcgen05_fence_before();
-  cluster_sync_all();   // nobody may exit (or free TMEM) while the peer can still touch its smem / barriers
-  if (warp == 2) {
-    tcgen05_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512) : "memory");
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// Host side: TMA descriptor encoding + launch
-// ------------------------------------------------------------------------------------------------
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
                                     const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                     const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -892,76 +400,33 @@ int make_tmap(CUtensorMap* tm, const void* base, long long inner, long long oute
   return MM_OK;
 }
 
-// experiment switches, read ONCE per process (never on the launch path)
-int env_group_m() {
+int env_group_m() {   // MM_GEMM_GM: rasterisation group size override (experiments; read once per process)
   static const int v = [] { const char* e = getenv("MM_GEMM_GM"); return e ? atoi(e) : 0; }();
-  return v;
-}
-int env_panel_mb() {   // MM_GEMM_PANEL_MB: L2 budget of the A panel of a rasterisation group (2-CTA kernel), default 32
-  static const int v = [] { const char* e = getenv("MM_GEMM_PANEL_MB"); return e ? atoi(e) : 32; }();
-  return v;
-}
-int env_dynamic_tiles() {   // MM_GEMM_DYNAMIC=0 selects the static persistent schedule of the 2-CTA kernel (A/B measurements)
-  static const int v = [] { const char* e = getenv("MM_GEMM_DYNAMIC"); return e ? atoi(e) : 1; }();
-  return v;
-}
-int env_tma_store() {   // MM_GEMM_TMA_STORE=0: direct st.global epilogue everywhere (A/B measurements)
-  static const int v = [] { const char* e = getenv("MM_GEMM_TMA_STORE"); return e ? atoi(e) : 1; }();
-  return v;
-}
-int env_l2_hint() {   // MM_GEMM_L2HINT=1 enables the TMA L2 eviction hints of the 2-CTA kernel. OFF by default: measured on B200
-  // (profiles/r02_gemm_ab.txt) they are neutral on the forward / dgrad shapes and cost 14-15 % on the wgrad
-  // ([28672 x 4096] = A^T B over 16384 tokens: 1323 vs 1542 TFLOP/s) and qkv (1276 vs 1503) shapes.
-  static const int v = [] { const char* e = getenv("MM_GEMM_L2HINT"); return e ? atoi(e) : 0; }();
   return v;
 }
 
 template <int BN, bool A_MN, bool B_MN>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, const EpiParams& ep,
            cudaStream_t stream) {
-  auto kern = gemm_tcgen05_kernel<BN, A_MN, B_MN>;
+  auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN>;
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
   std::call_once(once, [&] {
-    attr_err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    Cfg<BN>::kSmemBytes);
+    attr_err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::kSmemBytes);
   });
   MM_CHECK_CUDA(attr_err);
   const int num_tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
   const int grid = num_tiles < mm_num_sms() ? num_tiles : mm_num_sms();
-  // Rasterisation group (row-blocks per group), from the DRAM-traffic sweep in profiles/r01_gemm_raster_sweep.txt:
-  //  * a wave of concurrently running tiles should be "square" in bytes (gm*A_slab ~ gn*B_slab) so that every
-  //    k-slab fetched from HBM is shared by as many tiles as possible (lock-step sharing through L2): 17 row-blocks;
+  // Rasterisation group (row-blocks per group):
+  //  * a wave of concurrently running tiles should be about square in bytes so that every k-slab fetched from HBM
+  //    is shared by as many tiles as possible through L2: 132 SMs -> about 11 x 12 tiles;
   //  * when K is short the A panel of a group (gm * BM * K * 2 bytes) can stay L2-resident across the whole sweep
-  //    over N, so B is streamed once per group: take up to 32 MB (64 MB panels thrash: 4.9 GB vs 1.1 GB of reads).
-  long long gm = (32ll << 20) / ((long long)BM * K * 2);
-  if (gm < 17) gm = 17;
+  //    over N, so B is streamed once per group: up to 16 MB, a third of the H100's 50 MB L2.
+  long long gm = (16ll << 20) / ((long long)BM * K * 2);
+  if (gm < 11) gm = 11;
   if (gm > 64) gm = 64;
-  if (env_group_m() > 0) gm = env_group_m();   // rasterisation experiments (MM_GEMM_GM, read once)
+  if (env_group_m() > 0) gm = env_group_m();
   kern<<<grid, kThreads, Cfg<BN>::kSmemBytes, stream>>>(ta, tb, M, N, K, (int)gm, ep);
-  MM_CHECK_LAUNCH();
-  return MM_OK;
-}
-
-template <bool A_MN, bool B_MN, bool DYN>
-int launch2(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, int M, int N, int K, const EpiParams& ep,
-            cudaStream_t stream) {
-  auto kern = gemm_tcgen05_2cta_kernel<A_MN, B_MN, DYN>;
-  static std::once_flag once;
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [&] {
-    attr_err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem2Bytes);
-  });
-  MM_CHECK_CUDA(attr_err);
-  const int num_tiles = ((M + 2 * BM - 1) / (2 * BM)) * ((N + BN2 - 1) / BN2);
-  int clusters = mm_num_sms() / 2;
-  if (clusters > num_tiles || DYN) clusters = num_tiles;     // dynamic: one cluster per tile, the resident ones steal the rest
-  // same rule as the 1-CTA launcher with 256-row blocks and 74 concurrent cluster tiles (square wave: 8 x 9)
-  long long gm = ((long long)env_panel_mb() << 20) / ((long long)2 * BM * K * 2);
-  if (gm < 8) gm = 8;
-  if (gm > 32) gm = 32;
-  if (env_group_m() > 0) gm = env_group_m();   // rasterisation experiments (MM_GEMM_GM, read once)
-  kern<<<2 * clusters, kThreads, kSmem2Bytes, stream>>>(ta, tb, tc, M, N, K, (int)gm, env_l2_hint(), ep);
   MM_CHECK_LAUNCH();
   return MM_OK;
 }
@@ -1000,44 +465,10 @@ MM_API int mm_gemm_bf16(const void* A, const void* B, void* C, const void* bias,
                  "mm_gemm_bf16: SWIGLU aux alignment");
   }
   MM_CHECK_ARG(!(a_mn_major && !b_mn_major), "mm_gemm_bf16: (A MN-major, B K-major) not instantiated");
+  MM_CHECK_ARG(force_bn == 0 || force_bn == 128 || force_bn == 256, "mm_gemm_bf16: force_bn must be 0, 128 or 256 (got %d)",
+               force_bn);
 
-  // The 2-CTA (cta_group::2, 256x256 cluster tile) kernel is the default for problems with at least one full
-  // wave of cluster tiles: measured on B200 it sustains more under the power cap (train step 845.8 ms vs
-  // 866-869 ms with the 1-CTA kernel on the same box, profiles/r01_gemm_2cta_ab.txt) although its burst rate is
-  // lower. force_bn == 512 forces it, force_bn 128/256 or MM_GEMM_2CTA=0 select the 1-CTA kernel.
-  static const bool env_2cta = !(getenv("MM_GEMM_2CTA") != nullptr && atoi(getenv("MM_GEMM_2CTA")) == 0);
-  const long long tiles2 = ceil_div64(M, 2 * BM) * ceil_div64(N, BN2);
-  const bool use_2cta = (force_bn == 512) || (force_bn == 0 && env_2cta && tiles2 >= mm_num_sms() / 2);
-  if (use_2cta) {
-    CUtensorMap ta2, tb2;
-    int rc2;
-    if (!a_mn_major) rc2 = make_tmap(&ta2, A, K, M, lda, BK, BM);
-    else             rc2 = make_tmap(&ta2, A, M, K, lda, 64, BK);
-    if (rc2) return rc2;
-    if (!b_mn_major) rc2 = make_tmap(&tb2, B, K, N, ldb, BK, BN2 / 2);
-    else             rc2 = make_tmap(&tb2, B, N, K, ldb, 64, BK);
-    if (rc2) return rc2;
-    EpiParams ep2;
-    ep2.C = C; ep2.ldc = ldc;
-    ep2.bias = reinterpret_cast<const bf16*>(bias);
-    ep2.resid = reinterpret_cast<const bf16*>(resid); ep2.ldr = ldr;
-    ep2.aux = reinterpret_cast<bf16*>(aux); ep2.ld_aux = ld_aux;
-    ep2.epi = epilogue; ep2.out_f32 = out_f32; ep2.accumulate = accumulate; ep2.alpha = alpha;
-    // plain bf16 results (forward projections, dgrads, non-accumulating wgrads) leave through the TMA-store epilogue
-    ep2.tma_store = (env_tma_store() && !out_f32 && !accumulate && epilogue != EPI_SWIGLU && epilogue != EPI_SWIGLU_BWD) ? 1 : 0;
-    CUtensorMap tc2 = ta2;    // placeholder when unused (never dereferenced)
-    if (ep2.tma_store) {
-      if ((rc2 = make_tmap(&tc2, C, N, M, ldc, 64, BM))) return rc2;
-    }
-    if (env_dynamic_tiles()) {
-      if (!a_mn_major && !b_mn_major) return launch2<false, false, true>(ta2, tb2, tc2, (int)M, (int)N, (int)K, ep2, stream);
-      if (!a_mn_major && b_mn_major) return launch2<false, true, true>(ta2, tb2, tc2, (int)M, (int)N, (int)K, ep2, stream);
-      return launch2<true, true, true>(ta2, tb2, tc2, (int)M, (int)N, (int)K, ep2, stream);
-    }
-    if (!a_mn_major && !b_mn_major) return launch2<false, false, false>(ta2, tb2, tc2, (int)M, (int)N, (int)K, ep2, stream);
-    if (!a_mn_major && b_mn_major) return launch2<false, true, false>(ta2, tb2, tc2, (int)M, (int)N, (int)K, ep2, stream);
-    return launch2<true, true, false>(ta2, tb2, tc2, (int)M, (int)N, (int)K, ep2, stream);
-  }
+  // BN = 256 halves the B-operand traffic per flop; it needs a full wave of tiles to keep every SM busy.
   int bn = 256;
   if (force_bn == 128 || force_bn == 256) {
     bn = force_bn;
@@ -1061,7 +492,6 @@ MM_API int mm_gemm_bf16(const void* A, const void* B, void* C, const void* bias,
   ep.resid = reinterpret_cast<const bf16*>(resid); ep.ldr = ldr;
   ep.aux = reinterpret_cast<bf16*>(aux); ep.ld_aux = ld_aux;
   ep.epi = epilogue; ep.out_f32 = out_f32; ep.accumulate = accumulate; ep.alpha = alpha;
-  ep.tma_store = 0;
 
   const int m = (int)M, n = (int)N, k = (int)K;
   if (bn == 256) {

@@ -8,11 +8,14 @@
 //     row_map[r] <= -2           -> image_features[-(row_map[r]) - 2]        (projected visual token)
 //     row_map[r] == -1           -> zeros                                    (padding)
 // One warp moves one 8 KB row with coalesced 128-bit loads/stores (HBM-bound, 2*H bytes per row
-// read + written).  Backward scatters d(inputs_embeds) into the embedding-table gradient
-// (bf16x2 atomics: token ids repeat) and into d(image_features) (rows are unique: plain stores).
+// read + written).  Backward scatters d(inputs_embeds) into the embedding-table gradient and into d(image_features)
+// (rows are unique: plain stores). Token ids repeat: the warp of a token's FIRST row sums all of that token's rows in
+// row order in fp32 and stores once, so the embedding gradient is the same bits on every run (no atomics).
 #include "common.cuh"
 
 namespace {
+
+constexpr int kScatterVec = 8;   // 16-byte vectors per lane held in fp32 while one token's rows are summed
 
 __global__ void interleave_gather_kernel(const bf16* __restrict__ embed,
                                          const bf16* __restrict__ img,
@@ -62,12 +65,59 @@ __global__ void interleave_scatter_kernel(const bf16* __restrict__ dout,
       for (int v = lane; v < nvec; v += 32) dst[v] = ld_nc_int4(src + v);
     } else {
       if (dembed == nullptr) continue;
-      bf162* dst = reinterpret_cast<bf162*>(dembed + (size_t)m * H);
-      for (int v = lane; v < nvec; v += 32) {
-        const int4 g = ld_nc_int4(src + v);
-        const uint32_t u[4] = {(uint32_t)g.x, (uint32_t)g.y, (uint32_t)g.z, (uint32_t)g.w};
+      // only the first row carrying token m writes its gradient row
+      bool first = true;
+      for (long long r0 = 0; r0 < r && first; r0 += 32) {
+        const long long q = r0 + lane;
+        first = !__any_sync(0xffffffffu, q < r && row_map[q] == m);
+      }
+      if (!first) continue;
+      bf16* drow = dembed + (size_t)m * H;
+      for (int c0 = 0; c0 < nvec; c0 += 32 * kScatterVec) {   // kScatterVec 16-byte vectors per lane at a time
+        float acc[kScatterVec][8];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) atomicAdd(dst + v * 4 + j, *reinterpret_cast<const bf162*>(&u[j]));
+        for (int i = 0; i < kScatterVec; ++i) {
+          const int v = c0 + i * 32 + lane;
+          const int4 a = v < nvec ? reinterpret_cast<const int4*>(drow)[v] : make_int4(0, 0, 0, 0);
+          const uint32_t u[4] = {(uint32_t)a.x, (uint32_t)a.y, (uint32_t)a.z, (uint32_t)a.w};
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const float2 f = unpack_bf16x2(u[j]);
+            acc[i][2 * j] = f.x;
+            acc[i][2 * j + 1] = f.y;
+          }
+        }
+        for (long long r0 = r; r0 < R; r0 += 32) {
+          const long long q = r0 + lane;
+          unsigned hit = __ballot_sync(0xffffffffu, q < R && row_map[q] == m);
+          while (hit) {
+            const int b = __ffs(hit) - 1;
+            hit &= hit - 1;
+            const int4* g = reinterpret_cast<const int4*>(dout + (r0 + b) * H);
+#pragma unroll
+            for (int i = 0; i < kScatterVec; ++i) {
+              const int v = c0 + i * 32 + lane;
+              if (v < nvec) {
+                const int4 t = ld_nc_int4(g + v);
+                const uint32_t u[4] = {(uint32_t)t.x, (uint32_t)t.y, (uint32_t)t.z, (uint32_t)t.w};
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                  const float2 f = unpack_bf16x2(u[j]);
+                  acc[i][2 * j] += f.x;
+                  acc[i][2 * j + 1] += f.y;
+                }
+              }
+            }
+          }
+        }
+#pragma unroll
+        for (int i = 0; i < kScatterVec; ++i) {
+          const int v = c0 + i * 32 + lane;
+          if (v < nvec)
+            reinterpret_cast<int4*>(drow)[v] =
+                make_int4(pack_bf16x2(acc[i][0], acc[i][1]), pack_bf16x2(acc[i][2], acc[i][3]),
+                          pack_bf16x2(acc[i][4], acc[i][5]), pack_bf16x2(acc[i][6], acc[i][7]));
+        }
       }
     }
   }

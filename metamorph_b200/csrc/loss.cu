@@ -13,10 +13,51 @@ namespace {
 
 constexpr int kCEThreads = 512;
 
+// Loss sums are accumulated as fixed-point integers (integer addition is exact, so the total does not depend on the
+// order in which blocks finish); the last block of the launch converts the total and adds it to *loss_sum once.
+// Non-finite terms are not lost: NaN (or +Inf together with -Inf) makes the sum NaN, +/-Inf makes it +/-Inf, as a float
+// sum would. A finite term too large for the fixed-point range (`limit`, set so that no launch can overflow it) goes to
+// an fp64 side sum. The accumulator lives in per-stream scratch (mm_stream_scratch) and is reset by the last block.
+struct LossAcc {
+  unsigned long long fixed;
+  double big;
+  unsigned int blocks;
+  unsigned int flags;   // 1 NaN, 2 +Inf, 4 -Inf
+};
+
+__device__ __forceinline__ void loss_add(LossAcc* a, float v, double scale, float limit) {
+  if (isnan(v)) atomicOr(&a->flags, 1u);
+  else if (isinf(v)) atomicOr(&a->flags, v > 0.f ? 2u : 4u);
+  else if (fabsf(v) < limit) atomicAdd(&a->fixed, (unsigned long long)llrint((double)v * scale));
+  else atomicAdd(&a->big, (double)v);
+}
+// one thread per block, after every loss_add of the block
+__device__ __forceinline__ void loss_block_done(LossAcc* a, double scale, float* loss_sum) {
+  __threadfence();
+  if (atomicAdd(&a->blocks, 1u) == gridDim.x - 1) {
+    __threadfence();
+    const long long fixed = (long long)atomicExch(&a->fixed, 0ull);
+    const double big = __longlong_as_double((long long)atomicExch(reinterpret_cast<unsigned long long*>(&a->big), 0ull));
+    const unsigned int f = atomicExch(&a->flags, 0u);
+    a->blocks = 0;
+    float tot;
+    if ((f & 1u) || (f & 6u) == 6u) tot = NAN;
+    else if (f & 2u) tot = INFINITY;
+    else if (f & 4u) tot = -INFINITY;
+    else tot = (float)((double)fixed / scale + big);
+    *loss_sum += tot;
+  }
+}
+
+// fixed-point scales of the two sums; limit = 2^62 / (scale * rows) keeps every launch inside int64
+constexpr double kCEScale = 4294967296.0;            // 2^32: CE terms are O(10)
+constexpr double kCosScale = 1099511627776.0;        // 2^40: cosine terms are -cos/R, at most 1 in magnitude
+inline float loss_limit(double scale, long long rows) { return (float)(4611686018427387904.0 / (scale * (double)(rows > 0 ? rows : 1))); }
+
 __global__ void __launch_bounds__(kCEThreads)
 ce_fwd_bwd_kernel(const float* __restrict__ logits, long long ld, const int* __restrict__ labels,
-                  bf16* __restrict__ dlogits, long long ld_d, float* __restrict__ loss_sum,
-                  float* __restrict__ lse_out, int V, float grad_scale, int ignore_index) {
+                  bf16* __restrict__ dlogits, long long ld_d, float* __restrict__ loss_sum, LossAcc* __restrict__ acc,
+                  float limit, float* __restrict__ lse_out, int V, float grad_scale, int ignore_index) {
   __shared__ float red[32];
   const long long row = blockIdx.x;
   const float* x = logits + row * ld;
@@ -28,6 +69,7 @@ ce_fwd_bwd_kernel(const float* __restrict__ logits, long long ld, const int* __r
       for (long long j = threadIdx.x * 8; j < ld_d; j += kCEThreads * 8)
         *reinterpret_cast<int4*>(dx + j) = make_int4(0, 0, 0, 0);
     }
+    if (threadIdx.x == 0 && loss_sum != nullptr) loss_block_done(acc, kCEScale, loss_sum);
     return;
   }
   // pass 1: online max / sum(exp)
@@ -56,7 +98,10 @@ ce_fwd_bwd_kernel(const float* __restrict__ logits, long long ld, const int* __r
   const float lse = gm + logf(gs);
   if (threadIdx.x == 0) {
     if (lse_out != nullptr) lse_out[row] = lse;
-    if (valid && loss_sum != nullptr) atomicAdd(loss_sum, lse - x[label]);
+    if (loss_sum != nullptr) {
+      if (valid) loss_add(acc, lse - x[label], kCEScale, limit);
+      loss_block_done(acc, kCEScale, loss_sum);
+    }
   }
   if (dx == nullptr) return;
   // pass 2: gradient
@@ -81,8 +126,8 @@ ce_fwd_bwd_kernel(const float* __restrict__ logits, long long ld, const int* __r
 // one warp per row
 __global__ void cosine_loss_kernel(const bf16* __restrict__ pred, const bf16* __restrict__ target,
                                    bf16* __restrict__ pred_norm, bf16* __restrict__ dpred,
-                                   float* __restrict__ loss_sum, long long R, int C,
-                                   float grad_scale) {
+                                   float* __restrict__ loss_sum, LossAcc* __restrict__ acc, float limit,
+                                   long long R, int C, float grad_scale) {
   const int warps_per_block = blockDim.x >> 5;
   const int lane = threadIdx.x & 31;
   const int nvec = C >> 3;
@@ -132,7 +177,7 @@ __global__ void cosine_loss_kernel(const bf16* __restrict__ pred, const bf16* __
     hh = warp_sum(hh);
     const float tn = fmaxf(sqrtf(tt), 1e-8f), hn = fmaxf(sqrtf(hh), 1e-8f);
     const float cosv = tp / (tn * hn);
-    if (lane == 0 && loss_sum != nullptr) atomicAdd(loss_sum, -cosv / (float)R);
+    if (lane == 0 && loss_sum != nullptr) loss_add(acc, -cosv / (float)R, kCosScale, limit);
     if (dpred != nullptr) {
       // d(-mean cos)/d pred = -(1/R) * (t_hat - cos * p_hat) / |pred|
       const float g = -grad_scale / ((float)R * pn);
@@ -151,6 +196,10 @@ __global__ void cosine_loss_kernel(const bf16* __restrict__ pred, const bf16* __
         *reinterpret_cast<int4*>(dpred + r * C + v * 8) = make_int4(o[0], o[1], o[2], o[3]);
       }
     }
+  }
+  if (loss_sum != nullptr) {
+    __syncthreads();
+    if (threadIdx.x == 0) loss_block_done(acc, kCosScale, loss_sum);
   }
 }
 
@@ -209,9 +258,12 @@ MM_API int mm_ce_fwd_bwd(const float* logits, long long ld, const int* labels, v
                          float grad_scale, int ignore_index, cudaStream_t stream) {
   MM_CHECK_ARG(R > 0 && V > 0 && ld >= V && ld % 4 == 0, "mm_ce_fwd_bwd: need ld>=V and ld%%4==0");
   MM_CHECK_ARG(dlogits == nullptr || (ld_d >= V && ld_d % 8 == 0), "mm_ce_fwd_bwd: need ld_d>=V, ld_d%%8==0");
+  LossAcc* acc = nullptr;
+  if (loss_sum != nullptr && (acc = static_cast<LossAcc*>(mm_stream_scratch(MM_SCRATCH_LOSS, sizeof(LossAcc), stream))) == nullptr)
+    return MM_ERR_CUDA;
   ce_fwd_bwd_kernel<<<(unsigned)R, kCEThreads, 0, stream>>>(logits, ld, labels, (bf16*)dlogits, ld_d,
-                                                            loss_sum, lse_out, V, grad_scale,
-                                                            ignore_index);
+                                                            loss_sum, acc, loss_limit(kCEScale, R), lse_out, V,
+                                                            grad_scale, ignore_index);
   MM_CHECK_LAUNCH();
   return MM_OK;
 }
@@ -222,9 +274,12 @@ MM_API int mm_cosine_loss(const void* pred, const void* target, void* pred_norm,
   MM_CHECK_ARG(R > 0 && C % 8 == 0, "mm_cosine_loss: need C%%8==0");
   long long blocks = ceil_div64(R, 4);
   if (blocks > (long long)mm_num_sms() * 8) blocks = (long long)mm_num_sms() * 8;
+  LossAcc* acc = nullptr;
+  if (loss_sum != nullptr && (acc = static_cast<LossAcc*>(mm_stream_scratch(MM_SCRATCH_LOSS, sizeof(LossAcc), stream))) == nullptr)
+    return MM_ERR_CUDA;
   cosine_loss_kernel<<<(int)blocks, 128, 0, stream>>>((const bf16*)pred, (const bf16*)target,
-                                                      (bf16*)pred_norm, (bf16*)dpred, loss_sum, R, C,
-                                                      grad_scale);
+                                                      (bf16*)pred_norm, (bf16*)dpred, loss_sum, acc,
+                                                      loss_limit(kCosScale, R), R, C, grad_scale);
   MM_CHECK_LAUNCH();
   return MM_OK;
 }

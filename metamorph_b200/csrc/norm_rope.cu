@@ -82,7 +82,9 @@ rmsnorm_fwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, bf16*
 }
 
 // ---------------------------------------------------------------------------------- RMSNorm bwd
-// dx = dres_in + rstd*dy*w - x * rstd^3 * sum(dy*w*x)/H ;  dw += sum_rows dy * x * rstd  (fp32 atomics)
+// dx = dres_in + rstd*dy*w - x * rstd^3 * sum(dy*w*x)/H ;  dw += sum_rows dy * x * rstd
+// Every block stores its fp32 dw partial (the rows it owns) to a scratch row; rmsnorm_dw_reduce_kernel then adds the
+// partials in block order, so the weight gradient is the same bits on every run (no float atomics).
 // Both row statistics (sum x^2 and sum dy*w*x) come from ONE pass and ONE block reduction per row
 // (double-buffered smem scratch -> a single __syncthreads per row).
 // The loads of row r + gridDim.x (x, dy and the residual gradient: 6 of the 8 bytes per element the kernel moves) are
@@ -92,7 +94,7 @@ template <int VPT>   // 8-element vectors per thread (H <= 8 * 256 * VPT): sized
 __global__ void __launch_bounds__(kNormThreads, (VPT <= 2 ? 2 : 1))
 rmsnorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x,
                    const bf16* __restrict__ w, const bf16* __restrict__ dres_in,
-                   bf16* __restrict__ dx, float* __restrict__ dw_accum, int M, int H, float eps) {
+                   bf16* __restrict__ dx, float* __restrict__ dw_part, int M, int H, float eps) {
   __shared__ float red[2][2][kNormThreads / 32];
   const int nvec = H >> 3;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -178,19 +180,28 @@ rmsnorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x,
       }
     }
   }
-  if (dw_accum != nullptr) {
+  if (dw_part != nullptr) {
+    float* part = dw_part + (size_t)blockIdx.x * H;
 #pragma unroll
     for (int i = 0; i < VPT; ++i) {
       const int v = threadIdx.x + i * kNormThreads;
       if (v < nvec) {
-        // 128-bit reductions (red.global.add.v4.f32): a quarter of the L2 atomic operations of the scalar form — every
-        // block adds its 4096-wide partial into the same vector, so the tail of the kernel is atomic-throughput bound
-        atomicAdd(reinterpret_cast<float4*>(dw_accum + v * 8), make_float4(dwp[i][0], dwp[i][1], dwp[i][2], dwp[i][3]));
-        atomicAdd(reinterpret_cast<float4*>(dw_accum + v * 8 + 4), make_float4(dwp[i][4], dwp[i][5], dwp[i][6], dwp[i][7]));
+        *reinterpret_cast<float4*>(part + v * 8) = make_float4(dwp[i][0], dwp[i][1], dwp[i][2], dwp[i][3]);
+        *reinterpret_cast<float4*>(part + v * 8 + 4) = make_float4(dwp[i][4], dwp[i][5], dwp[i][6], dwp[i][7]);
       }
     }
   }
 }
+
+// dw[c] += sum over the n_part block partials of column c, in block order
+__global__ void rmsnorm_dw_reduce_kernel(const float* __restrict__ part, float* __restrict__ dw, int n_part, int H) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= H) return;
+  float s = 0.f;
+  for (int b = 0; b < n_part; ++b) s += part[(size_t)b * H + c];
+  dw[c] += s;
+}
+
 
 // ---------------------------------------------------------------------------------- LayerNorm fwd
 __global__ void __launch_bounds__(kNormThreads)
@@ -317,15 +328,24 @@ MM_API int mm_rmsnorm_bwd(const void* dy, const void* x, const void* w, const vo
   const int cap = mm_num_sms() * 4;       // 2 resident blocks per SM x 2 (tail balance)
   const int grid = M < cap ? (int)M : cap;
   const int vpt = (int)((H / 8 + kNormThreads - 1) / kNormThreads);
+  float* part = nullptr;
+  if (dw_accum != nullptr) {
+    part = static_cast<float*>(mm_stream_scratch(MM_SCRATCH_RMSNORM_DW, (size_t)grid * H * sizeof(float), stream));
+    if (part == nullptr) return MM_ERR_CUDA;
+  }
 #define MM_RMS_BWD(V)                                                                                      \
   rmsnorm_bwd_kernel<V><<<grid, kNormThreads, 0, stream>>>((const bf16*)dy, (const bf16*)x, (const bf16*)w, \
-                                                           (const bf16*)dres_in, (bf16*)dx, dw_accum, (int)M, \
+                                                           (const bf16*)dres_in, (bf16*)dx, part, (int)M, \
                                                            (int)H, eps)
   if (vpt <= 1) MM_RMS_BWD(1);
   else if (vpt == 2) MM_RMS_BWD(2);
   else MM_RMS_BWD(4);
 #undef MM_RMS_BWD
   MM_CHECK_LAUNCH();
+  if (dw_accum != nullptr) {
+    rmsnorm_dw_reduce_kernel<<<(unsigned)((H + 255) / 256), 256, 0, stream>>>(part, dw_accum, grid, (int)H);
+    MM_CHECK_LAUNCH();
+  }
   return MM_OK;
 }
 

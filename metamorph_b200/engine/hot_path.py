@@ -1,4 +1,4 @@
-"""The MetaMorph training/eval hot path on B200: vision tower -> projector -> gather-interleave ->
+"""The MetaMorph training/eval hot path on H100: vision tower -> projector -> gather-interleave ->
 LLaMA stack -> {lm_head + cross-entropy, vision_head + cosine regression} and the matching
 hand-written backward. Mirrors the data flow of the reference's
 `MetaMorphLlamaForCausalLM.forward` (metamorph_llama.py:603-660) = `prepare_inputs_labels_for_multimodal`

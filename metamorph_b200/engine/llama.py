@@ -1,4 +1,4 @@
-"""LLaMA decoder stack on the sm_100a kernels: explicit forward + hand-written backward.
+"""LLaMA decoder stack on the sm_90a kernels: explicit forward + hand-written backward.
 
 Arithmetic spec: HF `LlamaModel` (transformers modeling_llama.py: LlamaRMSNorm:53, rotary:73-168,
 LlamaMLP:171, LlamaAttention:225, LlamaDecoderLayer:292), called by the reference at

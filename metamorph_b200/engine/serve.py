@@ -5,7 +5,7 @@ The reference serves one request at a time (inference/demo.py:117-179: `generate
 embeddings). Here up to `max_slots` (<= 32) requests share every weight-streaming decode step:
   * each batch slot owns a KV-cache region, its mode / counters / position on the device and its own output limit;
   * a queued request is admitted into a free slot BETWEEN steps: its first P-1 prompt positions are prefilled with the
-    full-sequence kernels (tcgen05 GEMMs + flash attention) straight into the slot's cache region, and the last prompt
+    full-sequence kernels (wgmma GEMMs + flash attention) straight into the slot's cache region, and the last prompt
     position is fed through the ordinary decode step — no special first-token path;
   * the step itself (decoder stack + heads + argmax + state machine + next-input gather) is ONE captured CUDA graph
     replayed for all slots, exactly the kernels of DecodeEngine; idle / finished slots are frozen by the device state;

@@ -13,7 +13,7 @@ def load_pretrained_model(model_path, model_base, model_name, load_8bit=False, l
                           device_map="auto", device="cuda", use_flash_attn=False, torch_dtype=torch.float16,
                           **kwargs):
     if load_8bit or load_4bit:
-        raise NotImplementedError("quantised loading is out of scope for the B200 hot path")
+        raise NotImplementedError("quantised loading is out of scope for the H100 hot path")
     if "lora" in model_name.lower():
         raise NotImplementedError("LoRA checkpoints are out of scope (unused by the scripts)")
     if torch_dtype != torch.bfloat16:

@@ -1,5 +1,5 @@
 """Parameter-holding modules of the drop-in model. They carry the reference's parameter names
-(SURVEY.md §8b state-dict contract) but compute ONLY through the sm_100a kernels — there is no
+(SURVEY.md §8b state-dict contract) but compute ONLY through the sm_90a kernels — there is no
 eager/CPU fallback: calling them with CPU tensors raises (see _lib.require_cuda)."""
 from __future__ import annotations
 
@@ -13,7 +13,7 @@ from .. import ops
 
 
 class KernelLinear(nn.Module):
-    """nn.Linear-shaped parameter holder; forward = tcgen05 GEMM with a fused bias epilogue."""
+    """nn.Linear-shaped parameter holder; forward = wgmma GEMM with a fused bias epilogue."""
 
     def __init__(self, in_features: int, out_features: int, bias: bool = True, dtype=torch.bfloat16,
                  device=None, std: float = 0.02):

@@ -1,4 +1,4 @@
-"""Drop-in `MetaMorphLlamaForCausalLM` for the B200 hot path.
+"""Drop-in `MetaMorphLlamaForCausalLM` for the H100 hot path.
 
 Mirrors `metamorph/model/language_model/metamorph_llama.py`: `MetaMorphConfig` (:129),
 `MetaMorphLlamaModel` (:133), `MetaMorphLlamaForCausalLM` (:223) with `forward` (:603),
@@ -7,7 +7,7 @@ Mirrors `metamorph/model/language_model/metamorph_llama.py`: `MetaMorphConfig` (
 (`CausalLMOutputWithPast`, with `hidden_states` = last hidden state, not a tuple (:492-498)).
 
 Differences a caller can observe, all by design (DESIGN.md):
-  * compute runs only on CUDA sm_100a through the C-ABI kernels; CPU tensors raise (no fallback);
+  * compute runs only on CUDA sm_90a through the C-ABI kernels; CPU tensors raise (no fallback);
   * in training mode `logits` is None unless `config.output_logits_in_training` (the reference
     materialises an 8.4 GB fp32 [B,T,V] tensor each step; the fused head never does);
   * `loss.backward()` triggers the hand-written backward (no autograd graph through the stack);

@@ -1,4 +1,4 @@
-"""SigLIP vision tower on the sm_100a kernels (SURVEY.md rows A1, K1-K7).
+"""SigLIP vision tower on the sm_90a kernels (SURVEY.md rows A1, K1-K7).
 
 Mirrors `metamorph.model.multimodal_encoder.siglip_encoder.SiglipVisionTower` (siglip_encoder.py:62-213)
 for the configuration every reference script uses: SigLIP-SO400M/14@384 (hard-coded at :113),
@@ -142,7 +142,7 @@ class SiglipVisionTransformerParams(nn.Module):
         kpad = 640
         wpe = torch.zeros(c.hidden_size, kpad, dtype=pe.weight.dtype, device=pe.weight.device)
         wpe[:, :3 * c.patch_size * c.patch_size] = pe.weight.data.reshape(c.hidden_size, -1)
-        # Attention runs on the tcgen05 flash kernel (head_dim 128, csrc/attention_tc.cu): every head of width dh (72 for
+        # Attention runs on the wgmma flash kernel (head_dim 128, csrc/attention_tc.cu): every head of width dh (72 for
         # SO400M) is laid out in a 128-wide slot whose tail is exactly zero — zero rows in the fused QKV weight/bias, zero
         # columns in out_proj — so QK^T, softmax and the visible part of PV are those of the dh-wide heads
         # (HF modeling_siglip.py:229-249), with no pad/unpad pass over the activations.

@@ -6,12 +6,13 @@ from typing import Optional
 
 import torch
 
+from . import _lib
 from ._lib import c_float, c_int, c_void_p, call, ll, ptr, require_cuda, stream_ptr
 
 EPI_STORE, EPI_BIAS, EPI_BIAS_GELU_ERF, EPI_BIAS_GELU_TANH, EPI_RESID, EPI_BIAS_RESID, EPI_SWIGLU, EPI_SWIGLU_BWD = range(8)
 
 
-ATTN_BWD_TC = True  # tcgen05 backward (csrc/attention_tc.cu); the mma.sync kernel stays selectable with tc=False
+ATTN_BWD_TC = True  # wgmma backward (csrc/attention_bwd_tc.cu); the mma.sync kernel stays selectable with tc=False
 
 # bench.py instrumentation: when a list, every GEMM launch appends (start_event, end_event, flops)
 GEMM_PROFILE = None
@@ -27,7 +28,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
          resid: Optional[torch.Tensor] = None, aux: Optional[torch.Tensor] = None,
          epilogue: int = EPI_STORE, out_dtype: torch.dtype = torch.bfloat16,
          accumulate: bool = False, alpha: float = 1.0, force_bn: int = 0) -> torch.Tensor:
-    """bf16 tensor-core GEMM (tcgen05). Operand storage:
+    """bf16 tensor-core GEMM (wgmma). Operand storage:
          a_mn=False: a is [M, K] row-major;  a_mn=True: a is stored [K, M] row-major (A = a^T)
          b_mn=False: b is [N, K] row-major (C = A b^T, nn.Linear);  b_mn=True: b is [K, N] (C = A b)
     """
@@ -82,6 +83,8 @@ def rmsnorm_bwd(dy, x, w, eps, dres_in=None, dw_accum=None, out=None):
     out = torch.empty_like(x) if out is None else out
     call("mm_rmsnorm_bwd", ptr(dy), ptr(x), ptr(w), ptr(dres_in), ptr(out), ptr(dw_accum),
          ll(x.shape[0]), ll(x.shape[1]), c_float(eps), stream_ptr())
+    if dw_accum is not None:
+        _lib.launch_count += 1     # the in-order reduction of the weight-gradient partials
     return out
 
 
@@ -322,11 +325,11 @@ def attn_fwd(q, k, v, B, T, Hq, Hkv, head_dim, causal, scale, seqlens=None, out=
     if out is None:
         out = torch.empty((B * T, Hq * head_dim), dtype=torch.bfloat16, device=q.device)
     lse = torch.empty((B, Hq, T), dtype=torch.float32, device=q.device) if need_lse else None
-    # One kernel on the product path: tcgen05, 128-wide head slots (narrower heads are zero-padded into such slots by their
+    # One kernel on the product path: wgmma, 128-wide head slots (narrower heads are zero-padded into such slots by their
     # caller, as SiglipVisionTower does). tc=False selects the mma.sync comparison kernels (tests / microbenchmarks only).
     use_tc = True if tc is None else tc
     if use_tc and head_dim != 128:
-        raise ValueError(f"attn_fwd: the tcgen05 attention takes head_dim 128 (got {head_dim}); pad the heads into 128-wide "
+        raise ValueError(f"attn_fwd: the wgmma attention takes head_dim 128 (got {head_dim}); pad the heads into 128-wide "
                          "slots or pass tc=False for the mma.sync comparison kernel")
     call("mm_attn_fwd_tc" if use_tc else "mm_attn_fwd", ptr(q), ptr(k), ptr(v), ptr(out), ptr(lse), ptr(seqlens), ll(q.stride(0)),
          ll(k.stride(0)), ll(v.stride(0)), ll(out.stride(0)), c_int(B), c_int(T), c_int(Hq),
@@ -382,7 +385,7 @@ class SegmentTables:
 
 
 def attn_fwd_varlen(q, k, v, seg: SegmentTables, Hq, Hkv, head_dim, scale, out, need_lse=True):
-    """Block-diagonal causal attention over the packed sequences of `seg` in ONE launch (tcgen05 kernel).
+    """Block-diagonal causal attention over the packed sequences of `seg` in ONE launch (wgmma kernel).
     Rows outside every sequence are not written. Returns (out, lse [n_seg, Hq, max_len])."""
     require_cuda(q, k, v, out)
     assert q.stride(1) == 1 and k.stride(1) == 1 and v.stride(1) == 1 and head_dim == 128
@@ -439,8 +442,9 @@ def decode_attn(qkv, kcache, vcache, pos, cos, sin, Hq, Hkv, head_dim, scale, ou
     require_cuda(qkv, kcache, vcache, pos, cos, sin)
     B = qkv.shape[0]
     Tmax = kcache.shape[2]
-    if splits is None:  # enough CTAs to cover the SMs: B*Hkv*splits >= ~2 x 148
-        splits = max(1, min(16, -(-296 // (B * Hkv))))
+    if splits is None:  # enough CTAs to cover the SMs: B*Hkv*splits >= ~2 x #SMs
+        sms = torch.cuda.get_device_properties(qkv.device).multi_processor_count
+        splits = max(1, min(16, -(-2 * sms // (B * Hkv))))
     if out is None:
         out = torch.empty((B, Hq * head_dim), dtype=torch.bfloat16, device=qkv.device)
     ws = _workspace("decode_attn", B * Hkv * splits * (Hq // Hkv) * (2 + head_dim) * 4, qkv.device)

@@ -45,6 +45,11 @@ def test_bad_arguments_fail_loudly_without_gpu():
     with pytest.raises(MetaMorphB200Error, match="batch"):
         call("mm_skinny_gemm", c_void_p(0), c_void_p(0), c_void_p(0), c_void_p(0), c_void_p(0), ll(64), ll(64),
              ll(64), ll(0), c_int(33), c_int(64), c_int(64), c_int(0), c_int(0), c_void_p(0))
+    a = c_void_p(256)   # aligned, never dereferenced: the tile-width check rejects the call first
+    with pytest.raises(MetaMorphB200Error, match="force_bn"):
+        call("mm_gemm_bf16", a, a, a, c_void_p(0), c_void_p(0), c_void_p(0), ll(128), ll(128), ll(128), ll(128),
+             ll(128), ll(128), ll(0), ll(0), c_int(0), c_int(0), c_int(0), c_int(0), c_int(0), c_float(1.0), c_int(512),
+             c_void_p(0))
 
 
 def test_product_never_imports_oracle():

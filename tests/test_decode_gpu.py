@@ -1,4 +1,4 @@
-"""Decode kernels on B200 against torch fp32 restatements: skinny GEMM epilogues, split-context attention
+"""Decode kernels on H100 against torch fp32 restatements: skinny GEMM epilogues, split-context attention
 with RoPE + cache append, two-stage argmax, batched state machine vs the oracle loop."""
 import math
 

@@ -1,4 +1,4 @@
-"""Per-kernel parity tests (B200 only): each CUDA kernel, called through the C-ABI, against a plain
+"""Per-kernel parity tests (H100 only): each CUDA kernel, called through the C-ABI, against a plain
 torch fp32 restatement of the same op. Tolerances are bf16-level and written next to each check."""
 import math
 
@@ -34,12 +34,12 @@ def test_gemm_layouts(cuda_device, a_mn, b_mn, shape):
     a = torch.randn((K, M) if a_mn else (M, K), device=cuda_device).bfloat16()
     b = torch.randn((K, N) if b_mn else (N, K), device=cuda_device).bfloat16()
     ref = (a.float().t() if a_mn else a.float()) @ (b.float() if b_mn else b.float().t())
-    for bn in (128, 256, 512):   # 512 = 2-CTA (cta_group::2) kernel
+    for bn in (128, 256):   # both tile widths of the wgmma kernel
         out = ops.gemm(a, b, a_mn=a_mn, b_mn=b_mn, force_bn=bn)
         _close(out, ref, 1e-2, f"gemm bn={bn}")
 
 
-@pytest.mark.parametrize("force_bn", [0, 512])      # 512 = the 2-CTA kernel (TMA-store epilogue for plain bf16 results)
+@pytest.mark.parametrize("force_bn", [0, 256])      # 0 picks the 128-wide tile at this size; 256 forces the wide one
 def test_gemm_epilogues(cuda_device, force_bn):
     from metamorph_b200 import ops
     torch.manual_seed(1)
@@ -305,7 +305,7 @@ def _attn_ref(q, k, v, causal, scale, seqlens=None):
                                                  (2, 640, 4, 2, 128, False)])
 def test_attention_fwd(cuda_device, B, T, Hq, Hkv, d, causal, tc):
     if tc and d != 128:
-        pytest.skip("tcgen05 attention is specialised for head_dim 128")
+        pytest.skip("wgmma attention is specialised for head_dim 128")
     from metamorph_b200 import ops
     torch.manual_seed(10)
     qkv = torch.randn(B * T, (Hq + 2 * Hkv) * d, device=cuda_device).bfloat16()
@@ -360,7 +360,7 @@ def test_attention_bwd(cuda_device, B, T, Hq, Hkv, tc):
 
 
 def test_attention_bwd_tc_ignores_padded_dout_and_is_deterministic(cuda_device):
-    """The tcgen05 backward treats rows >= seqlens[b] as outside the sequence (the reference's masked positions carry no
+    """The wgmma backward treats rows >= seqlens[b] as outside the sequence (the reference's masked positions carry no
     gradient): a non-zero dO there must not change any result; and with no atomics two runs agree bit for bit."""
     from metamorph_b200 import ops
     torch.manual_seed(12)
@@ -420,3 +420,47 @@ def test_attention_varlen_packed_segments(cuda_device):
         _close(g[r0:r0 + n, Hq * d:(Hq + Hkv) * d].view(1, n, Hkv, d), kf.grad, 3e-2, f"varlen dk seg {r0}")
         _close(g[r0:r0 + n, (Hq + Hkv) * d:].view(1, n, Hkv, d), vf.grad, 3e-2, f"varlen dv seg {r0}")
     assert torch.all(out[~covered].float() == 7.0) and torch.all(g[~covered].float() == 3.0)   # gap rows untouched
+
+
+def test_loss_sums_carry_non_finite_terms_and_are_reproducible(cuda_device):
+    """The loss sums are order-independent (fixed point), yet a NaN term still makes the sum NaN and an Inf term makes
+    it Inf, as torch's cross-entropy / cosine losses report them; finite sums match torch and repeat bit for bit."""
+    from metamorph_b200 import ops
+    torch.manual_seed(3)
+    R, V = 64, 1000
+    logits = torch.randn(R, V, device=cuda_device) * 3
+    labels = torch.randint(0, V, (R,), device=cuda_device, dtype=torch.int32)
+    labels[5] = -100
+    ref = F.cross_entropy(logits, labels.long(), ignore_index=-100, reduction="sum").item()
+
+    def ce(lg):
+        s = torch.zeros(1, device=cuda_device)
+        ops.ce_fwd_bwd(lg, labels, V, s)
+        return s.item()
+
+    sums = [ce(logits) for _ in range(3)]
+    assert sums[0] == sums[1] == sums[2]
+    assert abs(sums[0] - ref) <= 1e-4 * abs(ref)
+    bad = logits.clone()
+    bad[7, 3] = float("nan")
+    assert math.isnan(ce(bad))
+    inf = logits.clone()
+    inf[9, int(labels[9])] = float("-inf")        # that row's term lse - x[label] is +Inf
+    assert ce(inf) == float("inf")
+    assert ce(logits) == sums[0]                  # a non-finite launch leaves the accumulator clean
+
+    pred = torch.randn(48, 1152, device=cuda_device).bfloat16()
+    tgt = torch.randn(48, 1152, device=cuda_device).bfloat16()
+
+    def cos(p):
+        s = torch.zeros(1, device=cuda_device)
+        ops.cosine_loss(p, tgt, loss_sum=s)
+        return s.item()
+
+    want = -F.cosine_similarity(pred.float(), tgt.float()).mean().item()
+    got = cos(pred)
+    assert got == cos(pred)
+    assert abs(got - want) <= 2e-3
+    pbad = pred.clone()
+    pbad[4, 10] = float("nan")
+    assert math.isnan(cos(pbad))

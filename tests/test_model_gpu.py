@@ -1,4 +1,4 @@
-"""Model-level parity on B200: the CUDA hot path (through the C-ABI) against (a) golden vectors made
+"""Model-level parity on H100: the CUDA hot path (through the C-ABI) against (a) golden vectors made
 by the reference itself (fp32 and bf16 runs, tests/golden/) and (b) the fp32 oracle restatement.
 
 Tolerances. The reference runs this path in bf16 with a rounding after every op; the fused kernels

@@ -1,4 +1,4 @@
-"""TrainEngine on B200: the fused (optimizer-in-backward) step, the clipped two-phase step and a plain
+"""TrainEngine on H100: the fused (optimizer-in-backward) step, the clipped two-phase step and a plain
 `loss.backward()` + torch.optim.AdamW loop must agree on the updated parameters."""
 import copy
 
