@@ -10,7 +10,7 @@
  *     mm_last_error() returns a thread-local message. No exceptions cross the ABI.
  *   - the caller owns every buffer (including workspaces); kernels never allocate or free.
  *   - all work is enqueued asynchronously on the given cudaStream_t; device pointers only.
- *   - mm_ce_fwd_bwd / mm_cosine_loss (with loss_sum) and mm_rmsnorm_bwd (with dw_accum) use library-owned device
+ *   - mm_ce_fwd_bwd / mm_cosine_loss (with loss_sum), mm_rmsnorm_bwd (with dw_accum) and mm_sumsq_bf16_accum use library-owned device
  *     scratch private to (device, stream), allocated on a stream's first such call: calls on one stream share it in
  *     stream order, calls on different streams never do. The first call on a stream must not be inside graph capture.
  *   - matrices are row-major bf16 unless stated; `ld*` are row pitches in elements.
@@ -60,6 +60,7 @@ int mm_gelu_bwd(const void* z, const void* da, void* dz, long long n, cudaStream
 int mm_colsum_accum(const void* x, float* out, long long R, long long N, long long ld, cudaStream_t s);
 int mm_im2col_patch14(const void* img, void* out, int n_img, int image_size, int ldp, cudaStream_t s);
 int mm_add_pos_emb(void* x, const void* pos, long long R, int P, int H, cudaStream_t s);
+/* *out += sum x^2 (two launches: per-block partials, then a fixed-order add, so the result is the same bits on every run). */
 int mm_sumsq_bf16_accum(const void* x, float* out, long long n, cudaStream_t s);
 
 /* Image/text token gather-interleave (metamorph_arch.py:272-399) and its backward.

@@ -51,7 +51,7 @@ int mm_num_sms();
 // it as they found it (or overwrite it fully), so stream-ordered calls can reuse it; calls on different streams never
 // share it. nullptr (with the error text set) when the allocation fails.
 void* mm_stream_scratch(int tag, size_t bytes, cudaStream_t stream);
-enum { MM_SCRATCH_LOSS = 0, MM_SCRATCH_RMSNORM_DW = 1 };
+enum { MM_SCRATCH_LOSS = 0, MM_SCRATCH_RMSNORM_DW = 1, MM_SCRATCH_SUMSQ = 2 };
 // programmatic dependent launch (PDL) for the decode chain: 1 unless MM_PDL=0 (api.cu)
 int mm_pdl_enabled();
 // MM_PDL_MODE bitmask (default 3): 1 = weight-streaming GEMMs launched with the PDL attribute, 2 = the small decode kernels

@@ -4,7 +4,7 @@
 //   colsum         : bias gradient (sum over rows)
 //   im2col_patch14 : SigLIP patch-embed Conv2d(k=s=14) as GEMM operand (modeling_siglip.py:178-184)
 //   add_pos_emb    : + learned position embedding
-//   sumsq / scale  : gradient-norm pieces for clipping
+//   sumsq          : squared gradient norm for clipping (per-block partials added in a fixed order by a second launch)
 #include "common.cuh"
 
 namespace {
@@ -152,7 +152,10 @@ __global__ void add_pos_emb_kernel(bf16* __restrict__ x, const bf16* __restrict_
   }
 }
 
-__global__ void sumsq_bf16_kernel(const bf16* __restrict__ x, float* __restrict__ out, long long n8) {
+// part[b] = sum of x^2 over the elements block b owns (grid-stride). Each thread adds its elements in order and the block
+// reduction has a fixed shape, so every partial is a function of (x, grid) only. No float atomics: sumsq_finish_kernel
+// adds the partials in a fixed order, so the gradient norm (and the clip coefficient) is the same bits on every run.
+__global__ void sumsq_bf16_kernel(const bf16* __restrict__ x, float* __restrict__ part, long long n8) {
   __shared__ float red[32];
   float s = 0.f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n8;
@@ -166,7 +169,21 @@ __global__ void sumsq_bf16_kernel(const bf16* __restrict__ x, float* __restrict_
     }
   }
   s = block_sum(s, red);
-  if (threadIdx.x == 0) atomicAdd(out, s);
+  if (threadIdx.x == 0) part[blockIdx.x] = s;
+}
+
+// *out += sum of the n_part partials. One warp: lane l adds partials l, l+32, l+64, ... in block order (fp64), then lane
+// 0 adds the 32 lane sums in lane order and rounds once to fp32.
+__global__ void sumsq_finish_kernel(const float* __restrict__ part, float* __restrict__ out, int n_part) {
+  __shared__ double lane_sum[32];
+  double s = 0.0;
+  for (int b = threadIdx.x; b < n_part; b += 32) s += (double)part[b];
+  lane_sum[threadIdx.x] = s;
+  __syncwarp();
+  if (threadIdx.x != 0) return;
+  double total = 0.0;
+  for (int l = 0; l < 32; ++l) total += lane_sum[l];
+  *out = (float)((double)*out + total);
 }
 
 int ew_grid(long long work_items, int threads) {
@@ -234,7 +251,12 @@ MM_API int mm_add_pos_emb(void* x, const void* pos, long long R, int P, int H, c
 
 MM_API int mm_sumsq_bf16_accum(const void* x, float* out, long long n, cudaStream_t stream) {
   MM_CHECK_ARG(n > 0 && n % 8 == 0, "mm_sumsq_bf16_accum: n%%8 != 0");
-  sumsq_bf16_kernel<<<ew_grid(n / 8, 256), 256, 0, stream>>>((const bf16*)x, out, n / 8);
+  const int grid = ew_grid(n / 8, 256);
+  float* part = static_cast<float*>(mm_stream_scratch(MM_SCRATCH_SUMSQ, (size_t)grid * sizeof(float), stream));
+  if (part == nullptr) return MM_ERR_CUDA;
+  sumsq_bf16_kernel<<<grid, 256, 0, stream>>>((const bf16*)x, part, n / 8);
+  MM_CHECK_LAUNCH();
+  sumsq_finish_kernel<<<1, 32, 0, stream>>>(part, out, grid);
   MM_CHECK_LAUNCH();
   return MM_OK;
 }

@@ -83,11 +83,13 @@ __global__ void adamw_kernel(bf16* __restrict__ p16, float* __restrict__ p32, fl
 }
 
 // out = min(1, max_norm / (sqrt(sumsq) + 1e-6))  (torch.nn.utils.clip_grad_norm_)
+// A NaN norm gives a NaN coefficient, as torch's clamp(max=1) does, so the update turns every parameter NaN instead of
+// applying the finite gradients unclipped. (fminf would return 1 for a NaN operand.)
 __global__ void clip_coef_kernel(const float* __restrict__ sumsq, float* __restrict__ out,
                                  float max_norm) {
   const float total = sqrtf(*sumsq);
   const float c = max_norm / (total + 1e-6f);
-  out[0] = c < 1.f ? c : 1.f;
+  out[0] = c >= 1.f ? 1.f : c;
   out[1] = total;
 }
 
