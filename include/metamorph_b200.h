@@ -89,6 +89,18 @@ int mm_cosine_loss(const void* pred, const void* target, void* pred_norm, void* 
 long long mm_argmax_workspace_bytes(long long R);
 int mm_argmax_rows(const float* logits, long long ld, long long R, int V, int* out, void* workspace,
                    long long workspace_bytes, cudaStream_t s);
+/* Seeded sampling in place of the argmax of metamorph_llama.py:542, one token per row, with HF's
+ * TemperatureLogitsWarper -> TopKLogitsWarper -> TopPLogitsWarper (transformers generation/logits_process.py) decided by
+ * value: z = l / T (NaN -> -inf); top-k keeps count(z_j > z_i) < k (ties kept; k <= 0 or k >= V: off); top-p keeps
+ * mass(z_j > z_i) < p * mass(top-k set) with mass_j = round(exp(z_j - max z) * 2^40) added as 64-bit integers (relative
+ * masses below ~1e-12 count as 0; p >= 1 or NaN: off; p <= 0: only the maximum). The token is the Gumbel-max
+ * argmax_i z_i - log(-log u_i) over the kept set, lowest index on ties, u_i = (w + 0.5) 2^-32 with w word (i & 3) of
+ * Philox4x32-10(counter (i >> 2, counter[r], 0, 0), key (seed[r] & 0xffffffff, seed[r] >> 32)): a pure function of the
+ * row's logits bits and parameters, the same on every run, under graph replay and whatever rows share the call.
+ * T <= 0 or NaN: exactly mm_argmax_rows' token. Always returns an index in [0, V) (0 for a row without a logit above
+ * -inf). Every per-row array is a device pointer. One launch of R thread-block clusters of 8 CTAs; V <= 393216. */
+int mm_sample_rows(const float* logits, long long ld, long long R, int V, const float* temperature, const int* top_k,
+                   const float* top_p, const unsigned long long* seed, const int* counter, int* out, cudaStream_t s);
 
 /* torch.optim.AdamW step (train.py:82 --optim adamw_torch), fused over flat buffers; clip coefficient. */
 int mm_adamw_step(void* p16, float* p32, float* m, float* v, const void* grad, int grad_f32, long long n, float lr,

@@ -1,4 +1,4 @@
-"""KV-cached greedy decode emitting text tokens and continuous visual-token embeddings.
+"""KV-cached greedy (or seeded sampled) decode emitting text tokens and continuous visual-token embeddings.
 
 Semantics = the reference's `greedy_decode` (metamorph_llama.py:502-597) including its quirks (EOS
 test on the logits of the overwritten hidden state while in image mode; the image-token counter is
@@ -8,7 +8,7 @@ only reset by <image_end>), but (a) with a KV cache instead of re-running the gr
 """
 from __future__ import annotations
 
-from typing import Optional
+from typing import Optional, Sequence, Union
 
 import torch
 
@@ -16,6 +16,7 @@ from .. import ops
 from ..constants import EOS_TOKEN_IDS, IMAGE_END_TOKEN_ID, IMAGE_START_TOKEN_ID
 from .decode_step import decode_heads, decoder_stack_step
 from .llama import StackContext
+from .sampling import SamplingArrays, SamplingParams, per_sequence
 
 
 class DecodeEngine:
@@ -28,8 +29,12 @@ class DecodeEngine:
                  max_new_tokens: int = 1024, start_image_token_id: int = IMAGE_START_TOKEN_ID,
                  end_image_token_id: int = IMAGE_END_TOKEN_ID, eos_token_id=EOS_TOKEN_IDS,
                  forced_tokens: Optional[torch.Tensor] = None, poll_every: int = 16,
-                 max_steps: Optional[int] = None):
+                 max_steps: Optional[int] = None,
+                 sampling: Union[None, SamplingParams, Sequence[SamplingParams]] = None):
         """inputs_embeds [B, P, H] (right-padded to P; prompt_lens[b] valid rows). B <= 32.
+        sampling: None (greedy), one SamplingParams (sequence b draws with seed + b) or one per sequence. The draw
+        replaces the argmax only: image mode, the EOS test on the drawn token and forced tokens are unchanged. When
+        every temperature is 0 this is the greedy path, kernel for kernel.
         Returns (ids list per sequence (int32 tensors), image_embeds list per sequence [n, C])."""
         m = self.m
         model = m.get_model()
@@ -38,6 +43,7 @@ class DecodeEngine:
         dev = inputs_embeds.device
         B, P, H = inputs_embeds.shape
         assert B <= 32, "decode batch is limited to 32 sequences per step (skinny GEMM: at most four n8 batch tiles)"
+        params = per_sequence(sampling, B)
         Hq, Hkv, dh = d.n_heads, d.n_kv_heads, d.head_dim
         L = len(model.layers)
         ntok = m.get_vision_tower().image_token_len if m.get_vision_tower() is not None else 0
@@ -80,12 +86,14 @@ class DecodeEngine:
         st["ids_out"] = torch.full((B, steps_cap + 1), -1, dtype=torch.int32, device=dev)
         img_out = torch.zeros((B, max_img, C), dtype=torch.bfloat16, device=dev)
         forced = forced_tokens.to(dev, dtype=torch.int32).contiguous() if forced_tokens is not None else None
+        samp = SamplingArrays.of(params, dev) if params is not None else None
         xin = torch.empty((B, H), dtype=torch.bfloat16, device=dev)
         V = m.lm_head.weight.shape[0]
         logits = torch.empty((B, (V + 7) // 8 * 8), dtype=torch.float32, device=dev)
 
         def heads_and_state(h_pre_norm, step):
-            tok, pred_z, prediction = decode_heads(m, h_pre_norm, st["in_image_mode"], logits, V)
+            tok, pred_z, prediction = decode_heads(m, h_pre_norm, st["in_image_mode"], logits, V, samp,
+                                                   st["total_output"])
             ops.decode_state_step(st, tok, forced, step, B, ntok, max_new_tokens, start_image_token_id,
                                   end_image_token_id, eos0, eos1, pred_z, img_out)
             ops.decode_next_input(st["append_kind"], st["next_token"], model.embed_tokens.weight.data,

@@ -1,6 +1,6 @@
 """The kernels of one KV-cached decode step, shared by DecodeEngine (one batch to completion) and
 ContinuousBatcher (a stream of requests): decoder stack on the weight-streaming GEMMs, then the heads
-(final norm, vision head -> projector feedback branch, lm_head, argmax). Reference arithmetic:
+(final norm, vision head -> projector feedback branch, lm_head, argmax or seeded draw). Reference arithmetic:
 metamorph_llama.py:363-377, 482-490 (decoding branch of llm_forward) and 526-582 (greedy_decode loop body)."""
 from __future__ import annotations
 
@@ -24,9 +24,11 @@ def decoder_stack_step(layers, x, kc, vc, cur_pos, stack):
     return x
 
 
-def decode_heads(m, h_pre_norm, in_image_mode, logits, V):
-    """-> (argmax token [B] int32, pred_z [B, C] (normalised visual embedding), prediction [B, H] (its projection)).
-    The image-mode branch is computed for every sequence and selected per sequence (graph friendly)."""
+def decode_heads(m, h_pre_norm, in_image_mode, logits, V, sampling=None, counter=None):
+    """-> (token [B] int32, pred_z [B, C] (normalised visual embedding), prediction [B, H] (its projection)).
+    The image-mode branch is computed for every sequence and selected per sequence (graph friendly).
+    sampling: None = argmax (metamorph_llama.py:542); else a SamplingArrays of per-row device parameters, and the token
+    is the seeded draw of ops.sample_rows with `counter` [B] int32 (steps each sequence has taken) on the device."""
     inner = m.get_model()
     d = m.stack.dims
     hidden = ops.rmsnorm(h_pre_norm, inner.norm.weight.data, d.rms_eps)
@@ -39,5 +41,8 @@ def decode_heads(m, h_pre_norm, in_image_mode, logits, V):
     h_eff = torch.empty_like(hidden)
     ops.decode_select_hidden(in_image_mode, hidden, prediction, h_eff)
     ops.skinny_gemm(h_eff, m.lm_head.weight.data, out=logits[:, :V])
-    tok = ops.argmax_rows(logits, V)
+    if sampling is None:
+        tok = ops.argmax_rows(logits, V)
+    else:
+        tok = ops.sample_rows(logits, V, sampling.temperature, sampling.top_k, sampling.top_p, sampling.seed, counter)
     return tok, pred_z, prediction

@@ -9,6 +9,10 @@ embeddings). Here up to `max_slots` (<= 32) requests share every weight-streamin
     position is fed through the ordinary decode step — no special first-token path;
   * the step itself (decoder stack + heads + argmax + state machine + next-input gather) is ONE captured CUDA graph
     replayed for all slots, exactly the kernels of DecodeEngine; idle / finished slots are frozen by the device state;
+  * a request may sample (`submit(..., sampling=SamplingParams(...))`): its slot's parameters and seed are written on
+    admission and the step counter is the slot's `total_output`. While a sampled request is in flight the step runs a
+    second graph, captured the first time it is needed, whose seeded draw replaces the argmax; a temperature-0 slot
+    gets the argmax token from it, so the graph choice never changes a greedy request's output;
   * the host polls the tiny state arrays every `poll_every` steps, hands out finished requests, streams the new text
     ids / visual embeddings of running ones (`run()` yields them), and refills the freed slots.
 Every request's output equals what `greedy_decode` produces for it alone (tests/test_decode_gpu.py).
@@ -25,6 +29,7 @@ from .. import ops
 from ..constants import EOS_TOKEN_IDS, IMAGE_END_TOKEN_ID, IMAGE_START_TOKEN_ID
 from .decode_step import decode_heads, decoder_stack_step
 from .llama import StackContext
+from .sampling import SamplingArrays, SamplingParams
 
 
 @dataclass
@@ -33,6 +38,7 @@ class _Request:
     embeds: torch.Tensor                 # [P, H] bf16 (device)
     max_new_tokens: int
     forced: Optional[torch.Tensor]       # [n] int32 (host) or None
+    sampling: Optional[SamplingParams] = None
     slot: int = -1
     sent_ids: int = 0
     sent_img: int = 0
@@ -86,46 +92,63 @@ class ContinuousBatcher:
         self.slots: List[Optional[_Request]] = [None] * B
         self.next_rid = 0
         self.steps_run = 0
-        self.graph = None
+        self.samp = SamplingArrays(B, dev)
+        self.graph = None                  # greedy step
+        self.sampled_graph = None          # step with the seeded draw, captured once a sampled request is in flight
         self.use_cuda_graph = use_cuda_graph
         self._warm = False
+        self._warm_sampled = False
 
     # ------------------------------------------------------------------ one device step for all slots
-    def _step_body(self):
+    def _step_body(self, sampled: bool = False):
         st = self.st
         x = decoder_stack_step(self.layers, self.xin, self.kc, self.vc, st["pos"] - 1, self.stack)
-        tok, pred_z, prediction = decode_heads(self.m, x, st["in_image_mode"], self.logits, self.V)
+        tok, pred_z, prediction = decode_heads(self.m, x, st["in_image_mode"], self.logits, self.V,
+                                               self.samp if sampled else None, st["total_output"])
         ops.decode_state_step_slots(st, tok, self.forced, self.max_new_slot, self.B, self.ntok, self.start_id,
                                     self.end_id, self.eos0, self.eos1, pred_z, self.img_out)
         ops.decode_next_input(st["append_kind"], st["next_token"], self.inner.embed_tokens.weight.data, prediction,
                               self.xin)
 
     def _device_step(self):
-        if self.graph is not None:
-            self.graph.replay()
-        elif self.use_cuda_graph and self._warm:
+        # the sampled step only while a sampled request holds a slot (finished slots are frozen: either step is fine)
+        sampled = any(r is not None and r.sampling is not None for r in self.slots)
+        graph = self.sampled_graph if sampled else self.graph
+        warm = self._warm_sampled if sampled else self._warm
+        if graph is not None:
+            graph.replay()
+        elif self.use_cuda_graph and warm:
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
             try:
                 with torch.cuda.graph(g):
-                    self._step_body()
-                self.graph = g                         # (the capture itself does not execute the step)
-                self.graph.replay()
+                    self._step_body(sampled)
+                if sampled:                            # (the capture itself does not execute the step)
+                    self.sampled_graph = g
+                else:
+                    self.graph = g
+                g.replay()
             except Exception:  # noqa: BLE001 - capture unsupported: stay on stream launches
                 self.use_cuda_graph = False
                 torch.cuda.synchronize()
-                self._step_body()
+                self._step_body(sampled)
         else:
-            self._step_body()                          # first step eager: sets kernel attributes
-            self._warm = True
+            self._step_body(sampled)                   # first step of each kind eager: sets kernel attributes
+            if sampled:
+                self._warm_sampled = True
+            else:
+                self._warm = True
         self.steps_run += 1
 
     # ------------------------------------------------------------------ requests
     @torch.no_grad()
     def submit(self, inputs_embeds: torch.Tensor, max_new_tokens: Optional[int] = None,
-               forced_tokens: Optional[torch.Tensor] = None) -> int:
+               forced_tokens: Optional[torch.Tensor] = None, sampling: Optional[SamplingParams] = None) -> int:
         """inputs_embeds: [P, H] or [1, P, H] prompt embeddings (text + projected image rows, as `generate` builds
-        them). Returns the request id."""
+        them). sampling: None or temperature 0 = greedy; otherwise the request draws its tokens with these parameters
+        and seed, and its output is the same whatever other requests share the server. Returns the request id."""
+        if sampling is not None and not isinstance(sampling, SamplingParams):
+            raise ValueError("sampling must be a SamplingParams or None")
         e = inputs_embeds.reshape(-1, inputs_embeds.shape[-1]).to(self.dev, dtype=torch.bfloat16).contiguous()
         n_new = self.cap if max_new_tokens is None else int(max_new_tokens)
         if n_new > self.cap:
@@ -135,7 +158,7 @@ class ContinuousBatcher:
         f = None if forced_tokens is None else forced_tokens.reshape(-1).to(torch.int32).cpu()
         rid = self.next_rid
         self.next_rid += 1
-        self.queue.append(_Request(rid, e, n_new, f))
+        self.queue.append(_Request(rid, e, n_new, f, sampling if sampling is not None and not sampling.greedy else None))
         return rid
 
     @torch.no_grad()
@@ -163,6 +186,7 @@ class ContinuousBatcher:
         self.st["append_kind"][b] = -1
         self.st["pos"][b] = P                       # the fed token sits at position P-1
         self.max_new_slot[b] = req.max_new_tokens
+        self.samp.set(b, req.sampling)
         req.slot, req.sent_ids, req.sent_img = b, 0, 0
         self.slots[b] = req
 

@@ -272,6 +272,22 @@ def argmax_rows(logits_f32, V, out=None):
     return out
 
 
+def sample_rows(logits_f32, V, temperature, top_k, top_p, seed, counter, out=None):
+    """One seeded draw per row from the temperature / top-k / top-p warped distribution (csrc/sampling.cu).
+    Per-row device arrays: temperature fp32, top_k int32, top_p fp32, seed int64 (the bits of a uint64), counter int32
+    (the number of steps the sequence has taken). Rows with temperature 0 get exactly argmax_rows' token."""
+    require_cuda(logits_f32, temperature, top_k, top_p, seed, counter, out)
+    R = logits_f32.shape[0]
+    assert logits_f32.dtype == torch.float32 and logits_f32.stride(1) == 1
+    for t, dt in ((temperature, torch.float32), (top_k, torch.int32), (top_p, torch.float32), (seed, torch.int64),
+                  (counter, torch.int32)):
+        assert t.dtype == dt and t.is_contiguous() and t.numel() >= R, "sample_rows: bad per-row array"
+    out = torch.empty((R,), dtype=torch.int32, device=logits_f32.device) if out is None else out
+    call("mm_sample_rows", ptr(logits_f32), ll(logits_f32.stride(0)), ll(R), c_int(V), ptr(temperature), ptr(top_k),
+         ptr(top_p), ptr(seed), ptr(counter), ptr(out), stream_ptr())
+    return out
+
+
 # ------------------------------------------------------------------------------------------------
 # optimizer
 # ------------------------------------------------------------------------------------------------
