@@ -179,6 +179,14 @@ int mm_siglip_preprocess(const void* img, int H, int W, int pad_square, int fill
 int mm_skinny_gemm(const void* x, const void* W, void* y, const void* bias, const void* resid, long long ldx,
                    long long ldw, long long ldy, long long ldr, int m, int N, int K, int epilogue, int out_f32,
                    cudaStream_t s);
+/* mm_skinny_gemm_wide: the same product, arguments and epilogues for 1 <= m <= 128 sequences (wgmma, K split over a
+ * thread-block cluster of up to 8 CTAs whose fp32 partials are added in rank order; no float atomics). The decode step
+ * calls it for m > 32. Determinism: a row's output bits depend only on its own x row, W, N, K and the epilogue (and its
+ * bias / residual row), never on m or the other rows, and repeated calls give the same bits. Against mm_skinny_gemm
+ * (m <= 32) the results agree within bf16 rounding, not bit for bit. */
+int mm_skinny_gemm_wide(const void* x, const void* W, void* y, const void* bias, const void* resid, long long ldx,
+                        long long ldw, long long ldy, long long ldr, int m, int N, int K, int epilogue, int out_f32,
+                        cudaStream_t s);
 long long mm_decode_attn_workspace_bytes(int B, int Hq, int Hkv, int splits);
 int mm_decode_attn(const void* qkv, long long ldqkv, void* kcache, void* vcache, const int* pos,
                    const float* cos_t, const float* sin_t, void* out, long long ldo, int B, int Hq, int Hkv,

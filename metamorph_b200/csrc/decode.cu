@@ -2,7 +2,7 @@
 //
 // The reference re-runs the whole prefix every step with no cache (metamorph_llama.py:510,526-535);
 // the mathematically equivalent cached step is HBM-bound: every weight byte is streamed once per
-// step for <= 32 sequences. Kernels:
+// step for <= 128 sequences (33..128 through skinny_gemm_wide, decode_wide.cu). Kernels:
 //   skinny_gemm   y[m<=32, N] = x[m, K] * W[N, K]^T : weight-streaming with mma.sync m16n8k16 where
 //                 the 16-row operand is a slab of W (rows = output features) and the 8-wide operand
 //                 is the batch (1, 2 or 4 n8 tiles). Weight slab and activation slice travel together

@@ -31,18 +31,19 @@ class DecodeEngine:
                  forced_tokens: Optional[torch.Tensor] = None, poll_every: int = 16,
                  max_steps: Optional[int] = None,
                  sampling: Union[None, SamplingParams, Sequence[SamplingParams]] = None):
-        """inputs_embeds [B, P, H] (right-padded to P; prompt_lens[b] valid rows). B <= 32.
+        """inputs_embeds [B, P, H] (right-padded to P; prompt_lens[b] valid rows). B <= 128.
         sampling: None (greedy), one SamplingParams (sequence b draws with seed + b) or one per sequence. The draw
         replaces the argmax only: image mode, the EOS test on the drawn token and forced tokens are unchanged. When
         every temperature is 0 this is the greedy path, kernel for kernel.
         Returns (ids list per sequence (int32 tensors), image_embeds list per sequence [n, C])."""
+        B, P, H = inputs_embeds.shape
+        assert B <= 128, f"decode batch is limited to 128 sequences per step (got {B}): the weight-streaming GEMM " \
+                         "serves at most 128 batch rows"
         m = self.m
         model = m.get_model()
         stack = m.stack
         d = stack.dims
         dev = inputs_embeds.device
-        B, P, H = inputs_embeds.shape
-        assert B <= 32, "decode batch is limited to 32 sequences per step (skinny GEMM: at most four n8 batch tiles)"
         params = per_sequence(sampling, B)
         Hq, Hkv, dh = d.n_heads, d.n_kv_heads, d.head_dim
         L = len(model.layers)

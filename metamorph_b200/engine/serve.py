@@ -2,7 +2,7 @@
 `greedy_decode` (metamorph_llama.py:502-597) for a stream of requests instead of one batch.
 
 The reference serves one request at a time (inference/demo.py:117-179: `generate` -> visualise the returned image
-embeddings). Here up to `max_slots` (<= 32) requests share every weight-streaming decode step:
+embeddings). Here up to `max_slots` (<= 128) requests share every weight-streaming decode step:
   * each batch slot owns a KV-cache region, its mode / counters / position on the device and its own output limit;
   * a queued request is admitted into a free slot BETWEEN steps: its first P-1 prompt positions are prefilled with the
     full-sequence kernels (wgmma GEMMs + flash attention) straight into the slot's cache region, and the last prompt
@@ -50,7 +50,7 @@ class ContinuousBatcher:
     def __init__(self, model, max_slots: int = 8, max_context: int = 2048, max_new_tokens: int = 1024,
                  poll_every: int = 8, use_cuda_graph: bool = True, start_image_token_id: int = IMAGE_START_TOKEN_ID,
                  end_image_token_id: int = IMAGE_END_TOKEN_ID, eos_token_id=EOS_TOKEN_IDS):
-        assert 1 <= max_slots <= 32, "the weight-streaming step serves at most 32 sequences"
+        assert 1 <= max_slots <= 128, f"the weight-streaming step serves at most 128 sequences (max_slots={max_slots})"
         self.m = model
         self.inner = model.get_model()
         self.stack = model.stack

@@ -440,15 +440,20 @@ ctypes_ll = _ctypes.c_longlong
 SK_STORE, SK_BIAS, SK_RESID, SK_BIAS_GELU, SK_SWIGLU = range(5)
 
 
-def skinny_gemm(x, w, *, bias=None, resid=None, epilogue=SK_STORE, out=None, out_dtype=torch.bfloat16):
-    """y[m<=32, N] = x[m, K] w[N, K]^T — HBM-bound weight streaming for the decode step (the batch is 1, 2 or 4 n8 MMA tiles)."""
+def skinny_gemm(x, w, *, bias=None, resid=None, epilogue=SK_STORE, out=None, out_dtype=torch.bfloat16, wide=None):
+    """y[m<=128, N] = x[m, K] w[N, K]^T — HBM-bound weight streaming for the decode step.
+    m <= 32 runs `mm_skinny_gemm` (mma.sync, the batch is 1, 2 or 4 n8 tiles); 33 <= m <= 128 runs `mm_skinny_gemm_wide`
+    (wgmma over a 128-wide batch operand, split-K reduced in a fixed order). The two agree within bf16 rounding; within one
+    kernel a row's bits do not depend on the other rows. `wide=True` forces the wide kernel for any m (comparisons)."""
     require_cuda(x, w, bias, resid, out)
     m, K = x.shape
     N = w.shape[0]
     n_out = N // 2 if epilogue == SK_SWIGLU else N
+    if wide is None:
+        wide = m > 32
     if out is None:
         out = torch.empty((m, n_out), dtype=out_dtype, device=x.device)
-    call("mm_skinny_gemm", ptr(x), ptr(w), ptr(out), ptr(bias), ptr(resid), ll(x.stride(0)),
+    call("mm_skinny_gemm_wide" if wide else "mm_skinny_gemm", ptr(x), ptr(w), ptr(out), ptr(bias), ptr(resid), ll(x.stride(0)),
          ll(w.stride(0)), ll(out.stride(0)), ll(resid.stride(0) if resid is not None else 0), c_int(m),
          c_int(N), c_int(K), c_int(epilogue), c_int(1 if out.dtype == torch.float32 else 0), stream_ptr())
     return out
