@@ -15,28 +15,13 @@ import math
 import pytest
 import torch
 
+from tests.exact import U, gamma as _gamma, ints as _ints, ulp_bf16 as _ulp_bf16
+
 pytestmark = pytest.mark.gpu
-
-U = 2.0 ** -24          # fp32 unit roundoff
-
-
-def _gamma(n):
-    """Higham's gamma_n: a sum evaluated along a chain of n fp32 additions is within gamma_n * sum|terms| of the exact sum."""
-    return n * U / (1 - n * U)
-
-
-def _ints(shape, lo, hi, device, dtype=torch.bfloat16, gen=None):
-    return torch.randint(lo, hi + 1, shape, device=device, generator=gen).to(dtype)
 
 
 def _sms(device):
     return torch.cuda.get_device_properties(device).multi_processor_count
-
-
-def _ulp_bf16(y):
-    """Spacing of bf16 numbers at |y| (8 significant bits): 2^(e - 8) for y = f * 2^e, 0.5 <= |f| < 1."""
-    _, e = torch.frexp(y.abs().float())
-    return torch.ldexp(torch.ones_like(y, dtype=torch.float64), e.to(torch.float64) - 8)
 
 
 # ------------------------------------------------------------------------------------------------ colsum (bias gradients)
