@@ -173,6 +173,12 @@ __device__ __forceinline__ float gelu_tanh(float x) {
 }
 __device__ __forceinline__ float silu(float x) { return x / (1.f + __expf(-x)); }
 
+// Rotate-half RoPE of the pair (a, b) = (x[j], x[j + d/2]): a c - b s and b c + a s. The rounded product and the fused
+// multiply-add are spelled out so that every kernel that rotates (rope_kernel, decode_attn_kernel) gets the same bits
+// whatever the compiler would contract: a prefilled K cache and a decoded one are identical.
+__device__ __forceinline__ float rope_lo(float a, float b, float c, float s) { return __fmaf_rn(a, c, -__fmul_rn(b, s)); }
+__device__ __forceinline__ float rope_hi(float a, float b, float c, float s) { return __fmaf_rn(b, c, __fmul_rn(a, s)); }
+
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");

@@ -236,15 +236,15 @@ decode_attn_kernel(const bf16* __restrict__ qkv, long long ldqkv, bf16* __restri
     const bf16* qh = row + (long long)(hk * G + h) * DA_D;
     const float a = __bfloat162float(qh[j]), c = __bfloat162float(qh[j + DA_D / 2]);
     // bf16 rounding of the rotated q mirrors the training kernel (rope_ writes bf16)
-    sq[h * DA_D + j] = __bfloat162float(__float2bfloat16(a * cp[j] - c * sp_[j])) * scale;
-    sq[h * DA_D + j + DA_D / 2] = __bfloat162float(__float2bfloat16(c * cp[j] + a * sp_[j])) * scale;
+    sq[h * DA_D + j] = __bfloat162float(__float2bfloat16(rope_lo(a, c, cp[j], sp_[j]))) * scale;
+    sq[h * DA_D + j + DA_D / 2] = __bfloat162float(__float2bfloat16(rope_hi(a, c, cp[j], sp_[j]))) * scale;
   }
   if (owns_new && tid < DA_D / 2) {
     const bf16* kh = row + (long long)(Hq + hk) * DA_D;
     const bf16* vh = row + (long long)(Hq + Hkv + hk) * DA_D;
     const float a = __bfloat162float(kh[tid]), c = __bfloat162float(kh[tid + DA_D / 2]);
-    const bf16 k0 = __float2bfloat16(a * cp[tid] - c * sp_[tid]);
-    const bf16 k1 = __float2bfloat16(c * cp[tid] + a * sp_[tid]);
+    const bf16 k0 = __float2bfloat16(rope_lo(a, c, cp[tid], sp_[tid]));   // the bits rope_ + kv_prefill would store
+    const bf16 k1 = __float2bfloat16(rope_hi(a, c, cp[tid], sp_[tid]));
     kcb[(long long)pos * DA_D + tid] = k0;
     kcb[(long long)pos * DA_D + tid + DA_D / 2] = k1;
     sknew[tid] = __bfloat162float(k0);

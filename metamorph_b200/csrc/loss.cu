@@ -205,7 +205,8 @@ __global__ void cosine_loss_kernel(const bf16* __restrict__ pred, const bf16* __
 
 // argmax over V fp32 logits per row, two stages so that a handful of rows still fills the GPU:
 // stage 1: grid (R, kArgmaxSplits) partial (value, index) per slice; stage 2: one warp per row.
-// Ties resolve to the smallest index (deterministic).
+// Ties resolve to the smallest index (deterministic). NaN never compares greater, so it is never chosen; a row with no
+// value above -inf (all -inf, all NaN, or a mix of the two) gives 0, as the sampler does, so the token is always in [0, V).
 constexpr int kArgmaxSplits = 64;
 
 __device__ __forceinline__ void argmax_combine(float& best, int& bi, float ov, int oi) {
@@ -248,7 +249,7 @@ __global__ void argmax_final_kernel(const float* __restrict__ pval, const int* _
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1)
     argmax_combine(best, bi, __shfl_xor_sync(0xffffffffu, best, o), __shfl_xor_sync(0xffffffffu, bi, o));
-  if (lane == 0) out[r] = bi;
+  if (lane == 0) out[r] = bi != 0x7fffffff ? bi : 0;
 }
 
 }  // namespace

@@ -288,8 +288,8 @@ __global__ void rope_kernel(bf16* __restrict__ qkv, const int* __restrict__ pos,
       const float2 b = unpack_bf16x2(uh[j]);
       const float c0 = cp[2 * j], c1 = cp[2 * j + 1];
       const float s0 = sign * sp[2 * j], s1 = sign * sp[2 * j + 1];
-      ol[j] = pack_bf16x2(a.x * c0 - b.x * s0, a.y * c1 - b.y * s1);
-      oh[j] = pack_bf16x2(b.x * c0 + a.x * s0, b.y * c1 + a.y * s1);
+      ol[j] = pack_bf16x2(rope_lo(a.x, b.x, c0, s0), rope_lo(a.y, b.y, c1, s1));
+      oh[j] = pack_bf16x2(rope_hi(a.x, b.x, c0, s0), rope_hi(a.y, b.y, c1, s1));
     }
     *reinterpret_cast<int4*>(p) = make_int4(ol[0], ol[1], ol[2], ol[3]);
     *reinterpret_cast<int4*>(p + half) = make_int4(oh[0], oh[1], oh[2], oh[3]);
