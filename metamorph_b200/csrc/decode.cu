@@ -438,10 +438,11 @@ __global__ void decode_state_kernel(DecodeState st, const int* __restrict__ argm
     int kind = -1;
     if (!st.finished[b]) {
       // forced schedule is indexed by this sequence's own step count (device-resident -> graph replayable)
-      const int fidx = st.total_output[b] < forced_ld ? st.total_output[b] : forced_ld - 1;
+      const int fidx = st.total_output[b];
       // a negative entry in the forced schedule means "free running" for that position (continuous batching mixes
-      // teacher-forced and free sequences in one batch)
-      const int ftok = forced ? forced[(long long)b * forced_ld + fidx] : -1;
+      // teacher-forced and free sequences in one batch), and so does every position past the schedule's last column:
+      // a schedule shorter than the run ends, it does not repeat its last token
+      const int ftok = (forced && fidx < forced_ld) ? forced[(long long)b * forced_ld + fidx] : -1;
       const int tok = ftok >= 0 ? ftok : argmax_tok[b];
       const int max_new = max_new_slot ? max_new_slot[b] : max_new_tokens;
       const int mode = st.in_image_mode[b];

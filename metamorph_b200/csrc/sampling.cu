@@ -6,6 +6,10 @@
 // load runs out of it: the row max, the fixed-point masses, the radix select of the top-k / top-p thresholds and the
 // Gumbel argmax. CTAs combine partial maxima and histograms through distributed shared memory; there is no global
 // workspace and no float atomic, so the token is a pure function of (logits bits, T, k, p, seed, counter).
+//
+// Rows without a usable scaled maximum never reach the draw: a row with no logit above -inf returns 0, and a row whose
+// max l / T is not finite (a +inf logit, or |max l| / T overflowing fp32 at a tiny T) returns the argmax of the logits,
+// lowest index among the maxima, whatever k, p and the seed are.
 #include <cooperative_groups.h>
 #include <math.h>
 #include <mutex>
@@ -229,12 +233,15 @@ sample_rows_kernel(const float* __restrict__ logits, long long ld, int V, int S,
 
   const float T = temperature[r];
   const bool greedy = !(T > 0.f);                        // T <= 0 or NaN
-  if (greedy || !(best > -INFINITY)) {                   // greedy, or no logit above -inf
-    if (rank == 0 && tid == 0) out[r] = (greedy && bi != 0x7fffffff) ? bi : 0;
+  const float zmax = best / T;
+  // Greedy, no logit above -inf, or max z = +-inf: a +inf logit, or a temperature so small that the divide overflows.
+  // Then z - max z is NaN or every scaled value collapses onto +-inf, and the row returns the limit T -> 0 of the draw:
+  // the argmax of the logits, lowest index among the maxima (bi is unset only when no logit is above -inf).
+  if (greedy || !(best > -INFINITY) || isinf(zmax)) {
+    if (rank == 0 && tid == 0) out[r] = bi != 0x7fffffff ? bi : 0;
     cluster.sync();                                      // keep this CTA's shared memory alive for the readers
     return;
   }
-  const float zmax = best / T;
   for (int j = tid; j < n; j += kSampleThreads) {
     const float v = zs[j];
     float z = isnan(v) ? -INFINITY : v / T;

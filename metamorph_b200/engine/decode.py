@@ -19,6 +19,20 @@ from .llama import StackContext
 from .sampling import SamplingArrays, SamplingParams, per_sequence
 
 
+def check_forced_tokens(forced_tokens: Optional[torch.Tensor], embed_rows: int) -> None:
+    """A forced id becomes a row index into the embedding table (the next-input gather reads row `id` unchecked), so
+    every entry must lie in [-1, embed_rows); -1 is free-running. Raises ValueError on the host, before any device
+    work."""
+    if forced_tokens is None or forced_tokens.numel() == 0:
+        return
+    if forced_tokens.dtype.is_floating_point or forced_tokens.dtype == torch.bool:
+        raise ValueError(f"forced_tokens must hold integer token ids (got {forced_tokens.dtype})")
+    lo, hi = int(forced_tokens.min()), int(forced_tokens.max())
+    if lo < -1 or hi >= embed_rows:
+        raise ValueError(f"forced_tokens must lie in [-1, {embed_rows}): -1 is free-running and an id indexes the "
+                         f"embedding table's {embed_rows} rows (got min {lo}, max {hi})")
+
+
 class DecodeEngine:
     def __init__(self, model):
         self.m = model
@@ -35,12 +49,19 @@ class DecodeEngine:
         sampling: None (greedy), one SamplingParams (sequence b draws with seed + b) or one per sequence. The draw
         replaces the argmax only: image mode, the EOS test on the drawn token and forced tokens are unchanged. When
         every temperature is 0 this is the greedy path, kernel for kernel.
+        forced_tokens: None or [B, n] integer ids indexed by each sequence's own step count. An entry >= 0 replaces the
+        step's token, -1 is free-running, and so is every step past column n - 1: a schedule shorter than the run ends
+        and the sequence free-runs from there, exactly as a request served by `ContinuousBatcher` does. Ids outside
+        [-1, embedding rows) raise ValueError before any device work.
         Returns (ids list per sequence (int32 tensors), image_embeds list per sequence [n, C])."""
         B, P, H = inputs_embeds.shape
         assert B <= 128, f"decode batch is limited to 128 sequences per step (got {B}): the weight-streaming GEMM " \
                          "serves at most 128 batch rows"
         m = self.m
         model = m.get_model()
+        if forced_tokens is not None and (forced_tokens.dim() != 2 or forced_tokens.shape[0] != B):
+            raise ValueError(f"forced_tokens must be [B={B}, n] (got {tuple(forced_tokens.shape)})")
+        check_forced_tokens(forced_tokens, model.embed_tokens.weight.shape[0])
         stack = m.stack
         d = stack.dims
         dev = inputs_embeds.device

@@ -15,7 +15,8 @@ embeddings). Here up to `max_slots` (<= 128) requests share every weight-streami
     gets the argmax token from it, so the graph choice never changes a greedy request's output;
   * the host polls the tiny state arrays every `poll_every` steps, hands out finished requests, streams the new text
     ids / visual embeddings of running ones (`run()` yields them), and refills the freed slots.
-Every request's output equals what `greedy_decode` produces for it alone (tests/test_decode_gpu.py).
+Every request's output equals what `greedy_decode` produces for it alone (tests/test_decode_gpu.py), a forced schedule
+shorter than the run included: in both, the request free-runs once its schedule ends (tests/test_serve_lifecycle_gpu.py).
 """
 from __future__ import annotations
 
@@ -27,6 +28,7 @@ import torch
 
 from .. import ops
 from ..constants import EOS_TOKEN_IDS, IMAGE_END_TOKEN_ID, IMAGE_START_TOKEN_ID
+from .decode import check_forced_tokens
 from .decode_step import decode_heads, decoder_stack_step
 from .llama import StackContext
 from .sampling import SamplingArrays, SamplingParams
@@ -146,7 +148,11 @@ class ContinuousBatcher:
                forced_tokens: Optional[torch.Tensor] = None, sampling: Optional[SamplingParams] = None) -> int:
         """inputs_embeds: [P, H] or [1, P, H] prompt embeddings (text + projected image rows, as `generate` builds
         them). sampling: None or temperature 0 = greedy; otherwise the request draws its tokens with these parameters
-        and seed, and its output is the same whatever other requests share the server. Returns the request id."""
+        and seed, and its output is the same whatever other requests share the server. forced_tokens: integer ids
+        indexed by the request's step count; an entry >= 0 replaces the step's token, -1 and every step past the
+        schedule's end are free-running (as in `DecodeEngine.generate`). Ids outside [-1, embedding rows) raise
+        ValueError here, before any device work. Returns the request id."""
+        check_forced_tokens(forced_tokens, self.inner.embed_tokens.weight.shape[0])
         if sampling is not None and not isinstance(sampling, SamplingParams):
             raise ValueError("sampling must be a SamplingParams or None")
         e = inputs_embeds.reshape(-1, inputs_embeds.shape[-1]).to(self.dev, dtype=torch.bfloat16).contiguous()

@@ -43,7 +43,8 @@ def gumbel_noise(V: int, seed: int, counter: int) -> np.ndarray:
 
 def scaled(logits, temperature: float) -> np.ndarray:
     """z = l / T in fp32 (IEEE divide), NaN -> -inf, returned as fp64."""
-    z = (np.asarray(logits, dtype=np.float32) / np.float32(temperature)).astype(np.float64)
+    with np.errstate(over="ignore", divide="ignore", invalid="ignore"):
+        z = (np.asarray(logits, dtype=np.float32) / np.float32(temperature)).astype(np.float64)
     z[np.isnan(z)] = -np.inf
     return z
 
@@ -75,13 +76,19 @@ def kept_set(z: np.ndarray, top_k: int, top_p: float):
 
 def draw(logits, temperature: float, top_k: int, top_p: float, seed: int, counter: int):
     """The sampled token of one row and the relative gap between its perturbed value and the runner-up
-    (inf when only one token is kept). T <= 0 is greedy: the lowest index of the maximum, NaN never chosen."""
+    (inf when only one token is kept). T <= 0 is greedy: the lowest index of the maximum, NaN never chosen. A row with
+    no logit above -inf gives 0; a row whose max l / T is not finite in fp32 gives the argmax as well."""
     logits = np.asarray(logits, dtype=np.float32)
     if not temperature > 0:
         return int(np.argmax(np.where(np.isnan(logits), -np.inf, logits))), np.inf, np.inf
-    z = scaled(logits, temperature)
-    if not (z > -np.inf).any():
+    clean = np.where(np.isnan(logits), np.float32(-np.inf), logits)
+    if not (clean > -np.inf).any():
         return 0, np.inf, np.inf
+    with np.errstate(over="ignore", divide="ignore"):
+        zmax = clean.max() / np.float32(temperature)
+    if np.isinf(zmax):          # a +inf logit, or |max l| / T beyond fp32: the limit T -> 0, the argmax, lowest index
+        return int(np.argmax(clean)), np.inf, np.inf
+    z = scaled(logits, temperature)
     keep, margin = kept_set(z, top_k, top_p)
     score = np.where(keep, z + gumbel_noise(z.shape[0], seed, counter), -np.inf)
     tok = int(np.argmax(score))
