@@ -194,6 +194,23 @@ int mm_decode_attn(const void* qkv, long long ldqkv, void* kcache, void* vcache,
                    cudaStream_t s);
 int mm_kv_prefill(const void* qkv, long long ld, void* kcache, void* vcache, int B, int T, int Hq, int Hkv,
                   int head_dim, int Tmax, cudaStream_t s);
+/* Paged KV cache. kpool / vpool (one pair per layer): [num_blocks, Hkv, block_size, 128] bf16; block_table:
+ * [B, max_blocks] int32 on the device, one row per sequence, shared by every layer. Logical position p of sequence b
+ * lives in block block_table[b * max_blocks + p / block_size] at row p % block_size. block_size is a power of two in
+ * [16, 256]. Every table entry the call can reach (those of positions 0..pos[b] for the attention, 0..T-1 for the
+ * prefill) must lie in [0, num_blocks); the kernels do not check them.
+ * mm_decode_attn_paged is mm_decode_attn with that addressing and the logical Tmax = max_blocks * block_size (which
+ * sizes the shared-memory bound exactly as in the dense call; workspace: mm_decode_attn_workspace_bytes). It walks
+ * the positions in the same split and order, so with equal splits its output and the appended K/V bits are those of
+ * mm_decode_attn on the same logical cache. mm_kv_prefill_paged copies the post-RoPE K/V rows of a prefill pass of
+ * ONE sequence (qkv rows [T, ld], positions 0..T-1) into the blocks of its table row (block_table_row points at that
+ * row); the bits are mm_kv_prefill's. */
+int mm_decode_attn_paged(const void* qkv, long long ldqkv, void* kpool, void* vpool, const int* block_table,
+                         int max_blocks, int block_size, const int* pos, const float* cos_t, const float* sin_t,
+                         void* out, long long ldo, int B, int Hq, int Hkv, int head_dim, float scale, void* workspace,
+                         long long workspace_bytes, int splits, cudaStream_t s);
+int mm_kv_prefill_paged(const void* qkv, long long ld, void* kpool, void* vpool, const int* block_table_row,
+                        int max_blocks, int block_size, int T, int Hq, int Hkv, int head_dim, cudaStream_t s);
 int mm_decode_state_step(int* in_image_mode, int* total_image_tokens, int* total_output, int* finished, int* pos,
                          int* n_ids, int* n_img, int* ids_out, int* append_kind, int* next_token,
                          const int* argmax_tok, const int* forced, int forced_ld, int step, int B,

@@ -201,15 +201,21 @@ skinny_gemm_tma_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
 // query heads of the group and writes partial (max, sum, unnormalised output); decode_attn_combine merges
 // the S partials. pos[b] = index of the new token; the CTA owning that position applies RoPE to the new k,
 // appends k/v to the cache and uses its on-chip copies (no cross-CTA read-after-write).
+// PAGED: kc / vc are block pools [num_blocks, Hkv, 1 << bs_shift, 128] and logical position p of sequence b lives in
+// block table[b * max_blocks + (p >> bs_shift)] at row p & (block_size - 1); Tmax = max_blocks << bs_shift. Only the
+// address of a K/V row changes: the split, the walk order and the arithmetic are the dense kernel's, so both give the
+// same bits on the same logical cache. The table row is read through the read-only path (one entry per position, L1
+// resident), which leaves the shared-memory footprint of the dense kernel unchanged.
 constexpr int DA_THREADS = 256;
 constexpr int DA_D = 128;
 
-template <int G>
+template <int G, bool PAGED>
 __global__ void __launch_bounds__(DA_THREADS)
 decode_attn_kernel(const bf16* __restrict__ qkv, long long ldqkv, bf16* __restrict__ kc,
                    bf16* __restrict__ vc, const int* __restrict__ pos_arr,
                    const float* __restrict__ cos_t, const float* __restrict__ sin_t,
-                   float* __restrict__ part, int Hq, int Hkv, int Tmax, int S, float scale) {
+                   float* __restrict__ part, int Hq, int Hkv, int Tmax, int S, float scale,
+                   const int* __restrict__ table, int max_blocks, int bs_shift) {
   extern __shared__ float sm[];
   float* sq = sm;                          // [G][128] rotated, scaled q
   float* sknew = sq + G * DA_D;            // [128] rotated new k
@@ -226,8 +232,18 @@ decode_attn_kernel(const bf16* __restrict__ qkv, long long ldqkv, bf16* __restri
   const int cpad = ((Tmax + S - 1) / S + 4) & ~3;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const bf16* row = qkv + (long long)b * ldqkv;
-  bf16* kcb = kc + ((long long)b * Hkv + hk) * Tmax * DA_D;
-  bf16* vcb = vc + ((long long)b * Hkv + hk) * Tmax * DA_D;
+  bf16* kcb = kc + (PAGED ? 0ll : ((long long)b * Hkv + hk) * Tmax * DA_D);
+  bf16* vcb = vc + (PAGED ? 0ll : ((long long)b * Hkv + hk) * Tmax * DA_D);
+  const int* trow = PAGED ? table + (long long)b * max_blocks : nullptr;
+  // element offset of the K/V row of logical position p, relative to kcb / vcb
+  auto row_off = [&](int p) -> long long {
+    if constexpr (PAGED) {
+      const long long blk = __ldg(trow + (p >> bs_shift));
+      return (((blk * Hkv + hk) << bs_shift) + (p & ((1 << bs_shift) - 1))) * DA_D;
+    } else {
+      return (long long)p * DA_D;
+    }
+  };
   const float* cp = cos_t + (long long)pos * (DA_D / 2);
   const float* sp_ = sin_t + (long long)pos * (DA_D / 2);
   const bool owns_new = (pos >= p0 && pos < p1);
@@ -245,13 +261,14 @@ decode_attn_kernel(const bf16* __restrict__ qkv, long long ldqkv, bf16* __restri
     const float a = __bfloat162float(kh[tid]), c = __bfloat162float(kh[tid + DA_D / 2]);
     const bf16 k0 = __float2bfloat16(rope_lo(a, c, cp[tid], sp_[tid]));   // the bits rope_ + kv_prefill would store
     const bf16 k1 = __float2bfloat16(rope_hi(a, c, cp[tid], sp_[tid]));
-    kcb[(long long)pos * DA_D + tid] = k0;
-    kcb[(long long)pos * DA_D + tid + DA_D / 2] = k1;
+    const long long ro = row_off(pos);
+    kcb[ro + tid] = k0;
+    kcb[ro + tid + DA_D / 2] = k1;
     sknew[tid] = __bfloat162float(k0);
     sknew[tid + DA_D / 2] = __bfloat162float(k1);
     const bf16 v0 = vh[2 * tid], v1 = vh[2 * tid + 1];
-    vcb[(long long)pos * DA_D + 2 * tid] = v0;
-    vcb[(long long)pos * DA_D + 2 * tid + 1] = v1;
+    vcb[ro + 2 * tid] = v0;
+    vcb[ro + 2 * tid + 1] = v1;
     svnew[2 * tid] = __bfloat162float(v0);
     svnew[2 * tid + 1] = __bfloat162float(v1);
   }
@@ -268,7 +285,7 @@ decode_attn_kernel(const bf16* __restrict__ qkv, long long ldqkv, bf16* __restri
         for (int h = 0; h < G; ++h) s[h] += sq[h * DA_D + d] * kf;
       }
     } else {
-      const int4* kp = reinterpret_cast<const int4*>(kcb + (long long)p * DA_D);
+      const int4* kp = reinterpret_cast<const int4*>(kcb + row_off(p));
 #pragma unroll 4
       for (int v = 0; v < DA_D / 8; ++v) {
         const int4 raw = kp[v];
@@ -328,7 +345,7 @@ decode_attn_kernel(const bf16* __restrict__ qkv, long long ldqkv, bf16* __restri
 #pragma unroll
           for (int j = 0; j < 4; ++j) vf[u][j] = svnew[lane * 4 + j];
         } else {
-          const uint2 raw = *reinterpret_cast<const uint2*>(vcb + (long long)p * DA_D + lane * 4);
+          const uint2 raw = *reinterpret_cast<const uint2*>(vcb + row_off(p) + lane * 4);
           const float2 f0 = unpack_bf16x2(raw.x), f1 = unpack_bf16x2(raw.y);
           vf[u][0] = f0.x; vf[u][1] = f0.y; vf[u][2] = f1.x; vf[u][3] = f1.y;
         }
@@ -404,6 +421,24 @@ __global__ void kv_prefill_kernel(const bf16* __restrict__ qkv, long long ld, bf
     const int t = (int)(r % T), b = (int)(r / T);
     const bf16* src = qkv + ((long long)b * T + t) * ld;
     const long long dst = (((long long)b * Hkv + hk) * Tmax + t) * DA_D + v * 8;
+    *reinterpret_cast<int4*>(kc + dst) = *reinterpret_cast<const int4*>(src + (long long)(Hq + hk) * DA_D + v * 8);
+    *reinterpret_cast<int4*>(vc + dst) = *reinterpret_cast<const int4*>(src + (long long)(Hq + Hkv + hk) * DA_D + v * 8);
+  }
+}
+
+// the same copy for one sequence into the blocks of its table row (pools [num_blocks, Hkv, 1 << bs_shift, 128])
+__global__ void kv_prefill_paged_kernel(const bf16* __restrict__ qkv, long long ld, bf16* __restrict__ kc,
+                                        bf16* __restrict__ vc, const int* __restrict__ trow, int T, int Hq, int Hkv,
+                                        int bs_shift) {
+  const long long total = (long long)T * Hkv * (DA_D / 8);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int v = (int)(i % (DA_D / 8));
+    const long long r = i / (DA_D / 8);
+    const int hk = (int)(r % Hkv), t = (int)(r / Hkv);
+    const bf16* src = qkv + (long long)t * ld;
+    const long long blk = __ldg(trow + (t >> bs_shift));
+    const long long dst = (((blk * Hkv + hk) << bs_shift) + (t & ((1 << bs_shift) - 1))) * DA_D + v * 8;
     *reinterpret_cast<int4*>(kc + dst) = *reinterpret_cast<const int4*>(src + (long long)(Hq + hk) * DA_D + v * 8);
     *reinterpret_cast<int4*>(vc + dst) = *reinterpret_cast<const int4*>(src + (long long)(Hq + Hkv + hk) * DA_D + v * 8);
   }
@@ -598,28 +633,32 @@ MM_API long long mm_decode_attn_workspace_bytes(int B, int Hq, int Hkv, int spli
   return (long long)B * Hkv * splits * (Hq / Hkv) * (2 + DA_D) * 4;
 }
 
-MM_API int mm_decode_attn(const void* qkv, long long ldqkv, void* kcache, void* vcache, const int* pos,
-                          const float* cos_t, const float* sin_t, void* out, long long ldo, int B,
-                          int Hq, int Hkv, int head_dim, int Tmax, float scale, void* workspace,
-                          long long workspace_bytes, int splits, cudaStream_t stream) {
-  MM_CHECK_ARG(head_dim == DA_D && Hq % Hkv == 0, "mm_decode_attn: need head_dim 128");
+namespace {
+
+// shared by the dense and the paged entry points; `name` prefixes the error messages. Dense: table == nullptr.
+template <bool PAGED>
+int decode_attn_launch(const char* name, const void* qkv, long long ldqkv, void* kcache, void* vcache, const int* pos,
+                       const float* cos_t, const float* sin_t, void* out, long long ldo, int B, int Hq, int Hkv,
+                       int head_dim, int Tmax, float scale, void* workspace, long long workspace_bytes, int splits,
+                       const int* table, int max_blocks, int bs_shift, cudaStream_t stream) {
+  MM_CHECK_ARG(head_dim == DA_D && Hq % Hkv == 0, "%s: need head_dim 128", name);
   const int G = Hq / Hkv;
-  MM_CHECK_ARG(G == 1 || G == 2 || G == 4 || G == 8, "mm_decode_attn: GQA group must be 1, 2, 4 or 8");
-  MM_CHECK_ARG(splits >= 1 && splits <= 64, "mm_decode_attn: splits in [1,64]");
+  MM_CHECK_ARG(G == 1 || G == 2 || G == 4 || G == 8, "%s: GQA group must be 1, 2, 4 or 8", name);
+  MM_CHECK_ARG(splits >= 1 && splits <= 64, "%s: splits in [1,64]", name);
   MM_CHECK_ARG(workspace != nullptr && workspace_bytes >= mm_decode_attn_workspace_bytes(B, Hq, Hkv, splits),
-               "mm_decode_attn: workspace too small");
+               "%s: workspace too small", name);
   const int cpad = ((Tmax + splits - 1) / splits + 4) & ~3;
   const size_t smem = (size_t)(G * DA_D + 2 * DA_D + 8 * G * DA_D + G * cpad) * sizeof(float);
-  MM_CHECK_ARG(smem <= 200 * 1024, "mm_decode_attn: Tmax/splits = %d positions per CTA is too large", cpad);
+  MM_CHECK_ARG(smem <= 200 * 1024, "%s: Tmax/splits = %d positions per CTA is too large", name, cpad);
   dim3 grid(Hkv, B, splits);
 #define MM_DA_LAUNCH(GG)                                                                                     \
   do {                                                                                                       \
     if (smem > 48 * 1024)                                                                                    \
-      MM_CHECK_CUDA(cudaFuncSetAttribute(decode_attn_kernel<GG>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                         (int)smem));                                                        \
-    MM_CHECK_CUDA(launch_pdl(mm_pdl_mode() & 2, decode_attn_kernel<GG>, grid, dim3(DA_THREADS), smem, stream, (const bf16*)qkv,  \
-                             ldqkv, (bf16*)kcache, (bf16*)vcache, pos, cos_t, sin_t, (float*)workspace, Hq,   \
-                             Hkv, Tmax, splits, scale));                                                     \
+      MM_CHECK_CUDA(cudaFuncSetAttribute(decode_attn_kernel<GG, PAGED>,                                      \
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));           \
+    MM_CHECK_CUDA(launch_pdl(mm_pdl_mode() & 2, decode_attn_kernel<GG, PAGED>, grid, dim3(DA_THREADS), smem, stream, \
+                             (const bf16*)qkv, ldqkv, (bf16*)kcache, (bf16*)vcache, pos, cos_t, sin_t,       \
+                             (float*)workspace, Hq, Hkv, Tmax, splits, scale, table, max_blocks, bs_shift));  \
   } while (0)
   if (G == 1) MM_DA_LAUNCH(1);
   else if (G == 2) MM_DA_LAUNCH(2);
@@ -629,6 +668,58 @@ MM_API int mm_decode_attn(const void* qkv, long long ldqkv, void* kcache, void* 
   MM_CHECK_LAUNCH();
   MM_CHECK_CUDA(launch_pdl(mm_pdl_mode() & 2, decode_attn_combine_kernel, dim3(Hkv, B), dim3(128), 0, stream, (const float*)workspace,
                            (bf16*)out, ldo, Hkv, G, splits));
+  MM_CHECK_LAUNCH();
+  return MM_OK;
+}
+
+// log2 of a block size in [16, 256], or -1
+int paged_block_shift(int block_size) {
+  if (block_size < 16 || block_size > 256 || (block_size & (block_size - 1))) return -1;
+  return __builtin_ctz((unsigned)block_size);
+}
+
+}  // namespace
+
+MM_API int mm_decode_attn(const void* qkv, long long ldqkv, void* kcache, void* vcache, const int* pos,
+                          const float* cos_t, const float* sin_t, void* out, long long ldo, int B,
+                          int Hq, int Hkv, int head_dim, int Tmax, float scale, void* workspace,
+                          long long workspace_bytes, int splits, cudaStream_t stream) {
+  return decode_attn_launch<false>("mm_decode_attn", qkv, ldqkv, kcache, vcache, pos, cos_t, sin_t, out, ldo, B, Hq,
+                                   Hkv, head_dim, Tmax, scale, workspace, workspace_bytes, splits, nullptr, 0, 0,
+                                   stream);
+}
+
+MM_API int mm_decode_attn_paged(const void* qkv, long long ldqkv, void* kpool, void* vpool, const int* block_table,
+                                int max_blocks, int block_size, const int* pos, const float* cos_t,
+                                const float* sin_t, void* out, long long ldo, int B, int Hq, int Hkv, int head_dim,
+                                float scale, void* workspace, long long workspace_bytes, int splits,
+                                cudaStream_t stream) {
+  const int shift = paged_block_shift(block_size);
+  MM_CHECK_ARG(shift >= 0, "mm_decode_attn_paged: block_size must be a power of two in [16,256] (got %d)", block_size);
+  MM_CHECK_ARG(max_blocks >= 1, "mm_decode_attn_paged: max_blocks must be >= 1 (got %d)", max_blocks);
+  MM_CHECK_ARG(block_table != nullptr, "mm_decode_attn_paged: block table missing");
+  MM_CHECK_ARG(Hkv >= 1, "mm_decode_attn_paged: need Hkv >= 1");
+  MM_CHECK_ARG((long long)max_blocks * block_size <= (1 << 30), "mm_decode_attn_paged: max_blocks too large");
+  return decode_attn_launch<true>("mm_decode_attn_paged", qkv, ldqkv, kpool, vpool, pos, cos_t, sin_t, out, ldo, B,
+                                  Hq, Hkv, head_dim, max_blocks * block_size, scale, workspace, workspace_bytes,
+                                  splits, block_table, max_blocks, shift, stream);
+}
+
+MM_API int mm_kv_prefill_paged(const void* qkv, long long ld, void* kpool, void* vpool, const int* block_table_row,
+                               int max_blocks, int block_size, int T, int Hq, int Hkv, int head_dim,
+                               cudaStream_t stream) {
+  const int shift = paged_block_shift(block_size);
+  MM_CHECK_ARG(shift >= 0, "mm_kv_prefill_paged: block_size must be a power of two in [16,256] (got %d)", block_size);
+  MM_CHECK_ARG(max_blocks >= 1, "mm_kv_prefill_paged: max_blocks must be >= 1 (got %d)", max_blocks);
+  MM_CHECK_ARG(block_table_row != nullptr, "mm_kv_prefill_paged: block table missing");
+  MM_CHECK_ARG(head_dim == DA_D && Hkv >= 1 && T >= 0 && (long long)T <= (long long)max_blocks * block_size,
+               "mm_kv_prefill_paged: need head_dim 128 and 0<=T<=max_blocks*block_size");
+  if (T == 0) return MM_OK;
+  const long long total = (long long)T * Hkv * (DA_D / 8);
+  long long blocks = ceil_div64(total, 256);
+  if (blocks > (long long)mm_num_sms() * 16) blocks = (long long)mm_num_sms() * 16;
+  kv_prefill_paged_kernel<<<(int)blocks, 256, 0, stream>>>((const bf16*)qkv, ld, (bf16*)kpool, (bf16*)vpool,
+                                                           block_table_row, T, Hq, Hkv, shift);
   MM_CHECK_LAUNCH();
   return MM_OK;
 }

@@ -9,14 +9,20 @@ import torch
 from .. import ops
 
 
-def decoder_stack_step(layers, x, kc, vc, cur_pos, stack):
-    """x [B, H] -> [B, H] through all layers; K/V of the fed position are appended to kc/vc [L, B, Hkv, Tmax, dh]."""
+def decoder_stack_step(layers, x, kc, vc, cur_pos, stack, table=None):
+    """x [B, H] -> [B, H] through all layers; K/V of the fed position are appended to kc/vc [L, B, Hkv, Tmax, dh].
+    With a block table [B, max_blocks] (int32, device) kc/vc are paged pools [L, num_blocks, Hkv, block_size, dh] and
+    the attention addresses them through it (ops.decode_attn_paged: the same bits as the dense cache)."""
     d = stack.dims
     Hq, Hkv, dh = d.n_heads, d.n_kv_heads, d.head_dim
     for i, w in enumerate(layers):
         n1 = ops.rmsnorm(x, w.ln1, d.rms_eps)
         qkv = ops.skinny_gemm(n1, w.wqkv)
-        attn = ops.decode_attn(qkv, kc[i], vc[i], cur_pos, stack.cos, stack.sin, Hq, Hkv, dh, stack.scale)
+        if table is None:
+            attn = ops.decode_attn(qkv, kc[i], vc[i], cur_pos, stack.cos, stack.sin, Hq, Hkv, dh, stack.scale)
+        else:
+            attn = ops.decode_attn_paged(qkv, kc[i], vc[i], table, cur_pos, stack.cos, stack.sin, Hq, Hkv, dh,
+                                         stack.scale)
         hmid = ops.skinny_gemm(attn, w.wo, resid=x, epilogue=ops.SK_RESID)
         n2 = ops.rmsnorm(hmid, w.ln2, d.rms_eps)
         act = ops.skinny_gemm(n2, w.wgu, epilogue=ops.SK_SWIGLU)

@@ -15,6 +15,10 @@ embeddings). Here up to `max_slots` (<= 128) requests share every weight-streami
     gets the argmax token from it, so the graph choice never changes a greedy request's output;
   * the host polls the tiny state arrays every `poll_every` steps, hands out finished requests, streams the new text
     ids / visual embeddings of running ones (`run()` yields them), and refills the freed slots.
+With `kv_pool_tokens` set, the slots share a paged KV cache instead of each reserving `max_context` positions: one pool
+of fixed-size blocks per layer and a device block table [max_slots, ceil(max_context / kv_block_size)] (see
+KVBlockAllocator for the reservation and reclaim rules). The paged attention kernel gives the dense one's bits, so a
+request's output does not depend on the cache layout or on which blocks it received.
 Every request's output equals what `greedy_decode` produces for it alone (tests/test_decode_gpu.py), a forced schedule
 shorter than the run included: in both, the request free-runs once its schedule ends (tests/test_serve_lifecycle_gpu.py).
 """
@@ -48,11 +52,64 @@ class _Request:
     img: List[torch.Tensor] = field(default_factory=list)
 
 
+class KVBlockAllocator:
+    """Host-side bookkeeping of the paged KV cache: which pool blocks are free and which request owns which.
+
+    Blocks 0 .. num_blocks-1 are handed out; block `scratch` (= num_blocks) never is. Every table entry of an idle
+    slot, and every entry past a request's reservation, points at the scratch block: idle and finished slots still
+    run every step and append K/V at their frozen position, and those writes must land where no request reads.
+
+    Reservation, not growth: a request gets on admission every block it can write. With P prompt positions and
+    max_new_tokens n, the prefill writes positions 0 .. P-2 and the decode state machine (decode_state_kernel) feeds
+    the token at pos-1, starting at pos = P and advancing pos once per step for at most n+1 steps; a finished slot
+    keeps rewriting its frozen position pos-1 = P+n until the host reclaims it. So positions 0 .. P+n are written and
+    read: ceil((P + n + 1) / block_size) blocks, never more (an early EOS only freezes the slot sooner)."""
+
+    def __init__(self, num_blocks: int, block_size: int):
+        check_kv_block_size(block_size)
+        if num_blocks < 1:
+            raise ValueError(f"a paged KV cache needs at least one block (num_blocks={num_blocks})")
+        self.num_blocks, self.block_size = num_blocks, block_size
+        self.scratch = num_blocks
+        self.free: List[int] = list(range(num_blocks))   # handed out from the front, returned to the back
+        self.owned: Dict[int, List[int]] = {}
+
+    def reservation(self, prompt_len: int, max_new_tokens: int) -> int:
+        """Blocks a request of `prompt_len` positions and `max_new_tokens` new tokens holds while it runs."""
+        return -(-(prompt_len + max_new_tokens + 1) // self.block_size)
+
+    def can_reserve(self, n_blocks: int) -> bool:
+        return n_blocks <= len(self.free)
+
+    def reserve(self, rid: int, n_blocks: int) -> List[int]:
+        assert rid not in self.owned, f"request {rid} already holds blocks"
+        assert self.can_reserve(n_blocks), f"{n_blocks} blocks requested, {len(self.free)} free"
+        blocks, self.free = self.free[:n_blocks], self.free[n_blocks:]
+        self.owned[rid] = blocks
+        return blocks
+
+    def release(self, rid: int) -> None:
+        self.free.extend(self.owned.pop(rid))
+
+
+def check_kv_block_size(block_size) -> None:
+    if not isinstance(block_size, int) or not 16 <= block_size <= 256 or block_size & (block_size - 1):
+        raise ValueError(f"kv_block_size must be a power of two in [16, 256] (got {block_size!r})")
+
+
 class ContinuousBatcher:
     def __init__(self, model, max_slots: int = 8, max_context: int = 2048, max_new_tokens: int = 1024,
                  poll_every: int = 8, use_cuda_graph: bool = True, start_image_token_id: int = IMAGE_START_TOKEN_ID,
-                 end_image_token_id: int = IMAGE_END_TOKEN_ID, eos_token_id=EOS_TOKEN_IDS):
+                 end_image_token_id: int = IMAGE_END_TOKEN_ID, eos_token_id=EOS_TOKEN_IDS,
+                 kv_pool_tokens: Optional[int] = None, kv_block_size: int = 64):
+        """kv_pool_tokens: None keeps one dense cache region of max_context positions per slot. An integer gives a
+        paged cache: a pool of ceil(kv_pool_tokens / kv_block_size) blocks (plus one scratch block) shared by all
+        slots; a request is admitted (strictly first come, first served) once a slot and the blocks it needs
+        are free. max_context stays the longest request either way."""
         assert 1 <= max_slots <= 128, f"the weight-streaming step serves at most 128 sequences (max_slots={max_slots})"
+        check_kv_block_size(kv_block_size)
+        if kv_pool_tokens is not None and (not isinstance(kv_pool_tokens, int) or kv_pool_tokens < 1):
+            raise ValueError(f"kv_pool_tokens must be None or a positive integer (got {kv_pool_tokens!r})")
         self.m = model
         self.inner = model.get_model()
         self.stack = model.stack
@@ -73,7 +130,16 @@ class ContinuousBatcher:
         self.eos1 = eos[1] if len(eos) > 1 else self.eos0
         self.start_id, self.end_id = start_image_token_id, end_image_token_id
         self.stack.ensure_positions(max_context + 1)
-        self.kc = torch.zeros((self.L, B, d.n_kv_heads, max_context, d.head_dim), dtype=torch.bfloat16, device=dev)
+        if kv_pool_tokens is None:
+            self.alloc, self.table = None, None
+            self.kc = torch.zeros((self.L, B, d.n_kv_heads, max_context, d.head_dim), dtype=torch.bfloat16, device=dev)
+        else:
+            self.alloc = KVBlockAllocator(-(-kv_pool_tokens // kv_block_size), kv_block_size)
+            self.max_blocks = -(-max_context // kv_block_size)
+            # pools [L, num_blocks + scratch, Hkv, block_size, dh]; table rows start (and return to) all scratch
+            self.kc = torch.zeros((self.L, self.alloc.num_blocks + 1, d.n_kv_heads, kv_block_size, d.head_dim),
+                                  dtype=torch.bfloat16, device=dev)
+            self.table = torch.full((B, self.max_blocks), self.alloc.scratch, dtype=torch.int32, device=dev)
         self.vc = torch.zeros_like(self.kc)
         self.st = {k: torch.zeros(B, dtype=torch.int32, device=dev) for k in
                    ("in_image_mode", "total_image_tokens", "total_output", "n_ids", "n_img", "append_kind",
@@ -104,7 +170,7 @@ class ContinuousBatcher:
     # ------------------------------------------------------------------ one device step for all slots
     def _step_body(self, sampled: bool = False):
         st = self.st
-        x = decoder_stack_step(self.layers, self.xin, self.kc, self.vc, st["pos"] - 1, self.stack)
+        x = decoder_stack_step(self.layers, self.xin, self.kc, self.vc, st["pos"] - 1, self.stack, self.table)
         tok, pred_z, prediction = decode_heads(self.m, x, st["in_image_mode"], self.logits, self.V,
                                                self.samp if sampled else None, st["total_output"])
         ops.decode_state_step_slots(st, tok, self.forced, self.max_new_slot, self.B, self.ntok, self.start_id,
@@ -151,16 +217,21 @@ class ContinuousBatcher:
         and seed, and its output is the same whatever other requests share the server. forced_tokens: integer ids
         indexed by the request's step count; an entry >= 0 replaces the step's token, -1 and every step past the
         schedule's end are free-running (as in `DecodeEngine.generate`). Ids outside [-1, embedding rows) raise
-        ValueError here, before any device work. Returns the request id."""
+        ValueError here, before any device work, and so does a request whose KV blocks exceed a paged server's whole
+        pool. Returns the request id."""
         check_forced_tokens(forced_tokens, self.inner.embed_tokens.weight.shape[0])
         if sampling is not None and not isinstance(sampling, SamplingParams):
             raise ValueError("sampling must be a SamplingParams or None")
-        e = inputs_embeds.reshape(-1, inputs_embeds.shape[-1]).to(self.dev, dtype=torch.bfloat16).contiguous()
+        P = inputs_embeds.reshape(-1, inputs_embeds.shape[-1]).shape[0]
         n_new = self.cap if max_new_tokens is None else int(max_new_tokens)
         if n_new > self.cap:
             raise ValueError(f"max_new_tokens {n_new} exceeds the server's limit {self.cap}")
-        if e.shape[0] < 1 or e.shape[0] + n_new + 2 > self.Tmax:
-            raise ValueError(f"prompt of {e.shape[0]} positions + {n_new} new ones does not fit max_context {self.Tmax}")
+        if P < 1 or P + n_new + 2 > self.Tmax:
+            raise ValueError(f"prompt of {P} positions + {n_new} new ones does not fit max_context {self.Tmax}")
+        if self.alloc is not None and self.alloc.reservation(P, n_new) > self.alloc.num_blocks:
+            raise ValueError(f"prompt of {P} positions + {n_new} new ones needs {self.alloc.reservation(P, n_new)} "
+                             f"KV blocks, more than the whole pool of {self.alloc.num_blocks}")
+        e = inputs_embeds.reshape(-1, inputs_embeds.shape[-1]).to(self.dev, dtype=torch.bfloat16).contiguous()
         f = None if forced_tokens is None else forced_tokens.reshape(-1).to(torch.int32).cpu()
         rid = self.next_rid
         self.next_rid += 1
@@ -172,6 +243,11 @@ class ContinuousBatcher:
         d = self.d
         Hq, Hkv, dh = d.n_heads, d.n_kv_heads, d.head_dim
         P = req.embeds.shape[0]
+        if self.alloc is not None:  # the slot's table row: its reserved blocks, then scratch
+            blocks = self.alloc.reserve(req.rid, self.alloc.reservation(P, req.max_new_tokens))
+            row = torch.full((self.max_blocks,), self.alloc.scratch, dtype=torch.int32)
+            row[:len(blocks)] = torch.tensor(blocks, dtype=torch.int32)
+            self.table[b].copy_(row.to(self.dev, non_blocking=True))
         if P > 1:   # prefill positions 0..P-2 into the slot's cache region
             pos = torch.arange(P - 1, dtype=torch.int32, device=self.dev)
             ctx = StackContext(B=1, T=P - 1, pos=pos, seqlens=None)
@@ -179,7 +255,10 @@ class ContinuousBatcher:
             for i, w in enumerate(self.layers):
                 x = self.stack.layer_forward(w, x, ctx, save=True, save_gu=False)
                 s = ctx.saved.pop()
-                ops.kv_prefill(s.qkv, self.kc[i, b:b + 1], self.vc[i, b:b + 1], 1, P - 1, Hq, Hkv, dh)
+                if self.alloc is None:
+                    ops.kv_prefill(s.qkv, self.kc[i, b:b + 1], self.vc[i, b:b + 1], 1, P - 1, Hq, Hkv, dh)
+                else:
+                    ops.kv_prefill_paged(s.qkv, self.kc[i], self.vc[i], self.table[b], P - 1, Hq, Hkv, dh)
                 del s
         self.xin[b].copy_(req.embeds[P - 1])
         row = torch.full((self.forced.shape[1],), -1, dtype=torch.int32)
@@ -195,6 +274,18 @@ class ContinuousBatcher:
         self.samp.set(b, req.sampling)
         req.slot, req.sent_ids, req.sent_img = b, 0, 0
         self.slots[b] = req
+
+    def _next_admission(self) -> Optional[int]:
+        """The lowest free slot if the queue head can be admitted now, else None. Strict FIFO: on a paged server a
+        head whose blocks are not free holds back every request behind it."""
+        if not self.queue:
+            return None
+        b = next((i for i, s in enumerate(self.slots) if s is None), None)
+        if b is not None and self.alloc is not None:
+            head = self.queue[0]
+            if not self.alloc.can_reserve(self.alloc.reservation(head.embeds.shape[0], head.max_new_tokens)):
+                return None
+        return b
 
     def _poll(self) -> Tuple[List[Tuple[int, str, torch.Tensor]], List[int]]:
         """One host sync: new ids / visual embeddings of every running request + the requests that finished."""
@@ -224,9 +315,10 @@ class ContinuousBatcher:
         (rid, 'done', (ids, image_embeds)) when a request completes. Returns when queue and slots are empty."""
         steps = 0
         while self.queue or any(s is not None for s in self.slots):
-            for b in range(self.B):
-                if self.slots[b] is None and self.queue:
-                    self._admit(self.queue.popleft(), b)
+            b = self._next_admission()
+            while b is not None:
+                self._admit(self.queue.popleft(), b)
+                b = self._next_admission()
             for _ in range(self.poll_every):
                 self._device_step()
                 steps += 1
@@ -236,6 +328,11 @@ class ContinuousBatcher:
             for b in done:
                 req = self.slots[b]
                 self.slots[b] = None
+                if self.alloc is not None:
+                    # the slot stays frozen, appending K/V at its last position every step: before the next step
+                    # (stream order) its row points at scratch, never at blocks another request may now receive
+                    self.alloc.release(req.rid)
+                    self.table[b].fill_(self.alloc.scratch)
                 ids = torch.cat(req.ids) if req.ids else torch.empty(0, dtype=torch.int32, device=self.dev)
                 img = torch.cat(req.img) if req.img else torch.empty((0, self.C), dtype=torch.bfloat16, device=self.dev)
                 yield (req.rid, "done", (ids, img))

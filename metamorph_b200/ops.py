@@ -459,13 +459,19 @@ def skinny_gemm(x, w, *, bias=None, resid=None, epilogue=SK_STORE, out=None, out
     return out
 
 
+def _decode_attn_splits(B, Hkv, device):
+    """Default context split of decode_attn / decode_attn_paged: enough CTAs to cover the SMs, B*Hkv*splits >= ~2 x
+    #SMs."""
+    sms = torch.cuda.get_device_properties(device).multi_processor_count
+    return max(1, min(16, -(-2 * sms // (B * Hkv))))
+
+
 def decode_attn(qkv, kcache, vcache, pos, cos, sin, Hq, Hkv, head_dim, scale, out=None, splits=None):
     require_cuda(qkv, kcache, vcache, pos, cos, sin)
     B = qkv.shape[0]
     Tmax = kcache.shape[2]
-    if splits is None:  # enough CTAs to cover the SMs: B*Hkv*splits >= ~2 x #SMs
-        sms = torch.cuda.get_device_properties(qkv.device).multi_processor_count
-        splits = max(1, min(16, -(-2 * sms // (B * Hkv))))
+    if splits is None:
+        splits = _decode_attn_splits(B, Hkv, qkv.device)
     if out is None:
         out = torch.empty((B, Hq * head_dim), dtype=torch.bfloat16, device=qkv.device)
     ws = _workspace("decode_attn", B * Hkv * splits * (Hq // Hkv) * (2 + head_dim) * 4, qkv.device)
@@ -479,6 +485,35 @@ def kv_prefill(qkv, kcache, vcache, B, T, Hq, Hkv, head_dim):
     require_cuda(qkv, kcache, vcache)
     call("mm_kv_prefill", ptr(qkv), ll(qkv.stride(0)), ptr(kcache), ptr(vcache), c_int(B), c_int(T),
          c_int(Hq), c_int(Hkv), c_int(head_dim), c_int(kcache.shape[2]), stream_ptr())
+
+
+def decode_attn_paged(qkv, kpool, vpool, table, pos, cos, sin, Hq, Hkv, head_dim, scale, out=None, splits=None):
+    """decode_attn over a paged cache: kpool / vpool [num_blocks, Hkv, block_size, head_dim], table [B, max_blocks]
+    int32 (device) mapping block p // block_size of sequence b to a pool block. With equal `splits` the output and the
+    appended K/V are bit-identical to decode_attn on the same logical cache of max_blocks * block_size positions."""
+    require_cuda(qkv, kpool, vpool, table, pos, cos, sin)
+    assert table.dtype == torch.int32 and table.dim() == 2 and table.is_contiguous(), "table: [B, max_blocks] int32"
+    B = qkv.shape[0]
+    assert table.shape[0] >= B
+    if splits is None:
+        splits = _decode_attn_splits(B, Hkv, qkv.device)
+    if out is None:
+        out = torch.empty((B, Hq * head_dim), dtype=torch.bfloat16, device=qkv.device)
+    ws = _workspace("decode_attn", B * Hkv * splits * (Hq // Hkv) * (2 + head_dim) * 4, qkv.device)
+    call("mm_decode_attn_paged", ptr(qkv), ll(qkv.stride(0)), ptr(kpool), ptr(vpool), ptr(table),
+         c_int(table.shape[1]), c_int(kpool.shape[2]), ptr(pos), ptr(cos), ptr(sin), ptr(out), ll(out.stride(0)),
+         c_int(B), c_int(Hq), c_int(Hkv), c_int(head_dim), c_float(scale), ptr(ws), ll(ws.numel()), c_int(splits),
+         stream_ptr())
+    return out
+
+
+def kv_prefill_paged(qkv, kpool, vpool, table_row, T, Hq, Hkv, head_dim):
+    """kv_prefill for one sequence into the blocks of its table row (table_row [max_blocks] int32, device)."""
+    require_cuda(qkv, kpool, vpool, table_row)
+    assert table_row.dtype == torch.int32 and table_row.dim() == 1 and table_row.stride(0) == 1
+    call("mm_kv_prefill_paged", ptr(qkv), ll(qkv.stride(0)), ptr(kpool), ptr(vpool), ptr(table_row),
+         c_int(table_row.shape[0]), c_int(kpool.shape[2]), c_int(T), c_int(Hq), c_int(Hkv), c_int(head_dim),
+         stream_ptr())
 
 
 def decode_state_step(st: dict, argmax_tok, forced, step, B, num_image_tokens, max_new_tokens,
