@@ -211,6 +211,18 @@ int mm_decode_attn_paged(const void* qkv, long long ldqkv, void* kpool, void* vp
                          long long workspace_bytes, int splits, cudaStream_t s);
 int mm_kv_prefill_paged(const void* qkv, long long ld, void* kpool, void* vpool, const int* block_table_row,
                         int max_blocks, int block_size, int T, int Hq, int Hkv, int head_dim, cudaStream_t s);
+/* Prefill attention over a paged cache (prefix caching: a suffix attends to shared prefix blocks). Causal flash attention
+ * of ONE sequence, head_dim 128, any GQA group, no lse: q [n_q, ldq] holds the query rows of positions
+ * q_start .. q_start + n_q - 1, and keys / values 0 .. kv_len - 1 (kv_len = q_start + n_q) are read from kpool / vpool
+ * [num_blocks, Hkv, block_size, 128] through block_table_row (max_blocks entries, same layout and block sizes as
+ * mm_decode_attn_paged; every entry of positions < kv_len must lie in [0, num_blocks)). o: [n_q, ldo]. Pool rows at or
+ * past kv_len are never used, whatever they hold (NaN included). Output row of position r is, bit for bit, row r of
+ * mm_attn_fwd_tc(B=1, T=kv_len, causal) on the same post-RoPE K/V: query tiles are aligned to absolute multiples of 128,
+ * so every row meets the same key tiles, masks and arithmetic as in the dense kernel. Arguments are checked (block
+ * size, table, head_dim, q_start >= 0, n_q >= 1, kv_len <= max_blocks * block_size, alignment) before any launch. */
+int mm_attn_fwd_tc_paged(const void* q, long long ldq, const void* kpool, const void* vpool, int num_blocks,
+                         const int* block_table_row, int max_blocks, int block_size, void* o, long long ldo,
+                         int q_start, int n_q, int Hq, int Hkv, int head_dim, float scale, cudaStream_t s);
 int mm_decode_state_step(int* in_image_mode, int* total_image_tokens, int* total_output, int* finished, int* pos,
                          int* n_ids, int* n_img, int* ids_out, int* append_kind, int* next_token,
                          const int* argmax_tok, const int* forced, int forced_ld, int step, int B,

@@ -9,6 +9,13 @@
 //                             are spread over the 4 lanes of a quad); P_j is packed to bf16 in place and is the
 //                             register A operand of O += P_j V_j (V MN-major from the same TMA tile).
 // The backward lives in attention_bwd_tc.cu.
+//
+// PAGED (mm_attn_fwd_tc_paged): the same kernel for ONE sequence whose keys / values sit in a paged KV pool
+// [num_blocks, Hkv, block_size, 128] addressed through a block-table row, and whose queries are the rows of positions
+// q_start .. q_start + n_q - 1 only. Query tiles stay aligned to absolute multiples of 128, so a row meets the key tiles,
+// mask decisions and consumer code of the dense kernel at T = q_start + n_q; the producer fills a 128-key tile with one
+// TMA box per block (the 128B swizzle repeats every 8 rows, so boxes of >= 16 rows land where one box would); V rows at or
+// past kv_len hold another request's data and are zeroed in shared memory, as the dense kernel's TMA zero fill would.
 #include "attention_tc.cuh"
 
 using namespace mm_attn_tc;
@@ -30,12 +37,21 @@ struct TcFwdParams {
   int causal;
 };
 
+// paged addressing (PAGED only): tmap_k / tmap_v cover the pool as [num_blocks * Hkv * block_size, 128] rows with
+// boxes of min(block_size, 128) rows; tmap_q covers the n_q query rows
+struct TcPagedParams {
+  const int* table;       // the sequence's block-table row
+  int q_start;            // absolute position of query row 0; kv_len = p.T = q_start + n_q
+  int bs_shift;           // log2(block_size)
+};
+
 constexpr int TC_THREADS = 384;
 constexpr int TC_SMEM = 5 * TC_TILE_BYTES + 256 + 1024;
 
+template <bool PAGED>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 flash_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                       const __grid_constant__ CUtensorMap tmap_v, TcFwdParams p) {
+                       const __grid_constant__ CUtensorMap tmap_v, TcFwdParams p, TcPagedParams pg) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sQ = base;
@@ -48,7 +64,8 @@ flash_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   // padded batch: grid = (query tiles, heads, sequences), heavy (late) tiles first; packed sequences (SURVEY 8f N2):
   // grid.x walks a host-built list of the (sequence, query tile) pairs that exist, one launch for all segments
-  const int qt = p.work ? p.work[blockIdx.x].y : (int)gridDim.x - 1 - (int)blockIdx.x;
+  int qt = p.work ? p.work[blockIdx.x].y : (int)gridDim.x - 1 - (int)blockIdx.x;
+  if constexpr (PAGED) qt += pg.q_start / TC_BR;        // absolute tiles from the one holding q_start
   const int h = blockIdx.y, b = p.work ? p.work[blockIdx.x].x : (int)blockIdx.z;
   const int hk = h / (p.Hq / p.Hkv);
   const int q0 = qt * TC_BR;
@@ -78,13 +95,52 @@ flash_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
     setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
       if (n_tiles > 0) {
+        // paged: the operand holds rows q_start.. only; rows before it (negative coordinates) arrive as zero fill
+        const int qrow = PAGED ? q0 - pg.q_start : tok0 + q0;
         mbar_arrive_expect_tx(q_full, TC_TILE_BYTES);
-        tma_load_2d(sQ, &tmap_q, q_full, h * TC_D, tok0 + q0);
-        tma_load_2d(sQ + 16384, &tmap_q, q_full, h * TC_D + 64, tok0 + q0);
+        tma_load_2d(sQ, &tmap_q, q_full, h * TC_D, qrow);
+        tma_load_2d(sQ + 16384, &tmap_q, q_full, h * TC_D + 64, qrow);
       }
       for (int j = 0; j < n_tiles; ++j) {
         const int bf = j & 1;
         const uint32_t ph = (uint32_t)((j >> 1) & 1);
+        if constexpr (PAGED) {
+          // one box of sb rows per block; boxes starting at or past kv_len are not loaded (their keys are masked and
+          // their values zeroed by the consumers)
+          const int sb = min(TC_BC, 1 << pg.bs_shift), kv0 = j * TC_BC;
+          const int nbox = (min(TC_BC, kv_len - kv0) + sb - 1) / sb;
+          const uint32_t bytes = (uint32_t)(nbox * sb * 256);
+          int prow[8];
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            if (i < nbox) {
+              const int pos = kv0 + i * sb;
+              const int blk = __ldg(pg.table + (pos >> pg.bs_shift));
+              prow[i] = ((blk * p.Hkv + hk) << pg.bs_shift) + (pos & ((1 << pg.bs_shift) - 1));
+            }
+          }
+          mbar_wait(bf ? k_empty1 : k_empty0, ph ^ 1);
+          mbar_arrive_expect_tx(bf ? k_full1 : k_full0, bytes);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            if (i < nbox) {
+              const uint32_t off = (uint32_t)(i * sb * 128);
+              tma_load_2d(sK[bf] + off, &tmap_k, bf ? k_full1 : k_full0, 0, prow[i]);
+              tma_load_2d(sK[bf] + 16384 + off, &tmap_k, bf ? k_full1 : k_full0, 64, prow[i]);
+            }
+          }
+          mbar_wait(bf ? v_empty1 : v_empty0, ph ^ 1);
+          mbar_arrive_expect_tx(bf ? v_full1 : v_full0, bytes);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            if (i < nbox) {
+              const uint32_t off = (uint32_t)(i * sb * 128);
+              tma_load_2d(sV[bf] + off, &tmap_v, bf ? v_full1 : v_full0, 0, prow[i]);
+              tma_load_2d(sV[bf] + 16384 + off, &tmap_v, bf ? v_full1 : v_full0, 64, prow[i]);
+            }
+          }
+          continue;
+        }
         mbar_wait(bf ? k_empty1 : k_empty0, ph ^ 1);
         mbar_arrive_expect_tx(bf ? k_full1 : k_full0, TC_TILE_BYTES);
         tma_load_2d(sK[bf], &tmap_k, bf ? k_full1 : k_full0, hk * TC_D, tok0 + j * TC_BC);
@@ -157,6 +213,21 @@ flash_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
 #pragma unroll
     for (int k = 0; k < TC_BC / 16; ++k) acc_to_a(sacc, k, pa[k]);
     mbar_wait(bf ? v_full1 : v_full0, ph);
+    if constexpr (PAGED) {
+      // The tile straddling kv_len (the CTA's last, at most once): pool rows past kv_len are stale, possibly NaN, and
+      // 0 * NaN would poison O. Zero them in both 64-column halves, as the dense kernel's TMA zero fill leaves them, then
+      // make the generic-proxy stores visible to wgmma and wait for both consumer warpgroups.
+      const int valid = kv_len - j * TC_BC;
+      if (valid < TC_BC) {
+        for (int idx = (int)threadIdx.x - 128; idx < (TC_BC - valid) * 16; idx += 256) {
+          const uint32_t a = sV[bf] + (uint32_t)(idx & 8) * 2048u + (uint32_t)(valid + (idx >> 4)) * 128u +
+                             (uint32_t)(idx & 7) * 16u;
+          asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(a), "r"(0u) : "memory");
+        }
+        fence_proxy_async_smem();
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+      }
+    }
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < TC_BC / 16; ++k) wgmma_m64n128_rs<1>(o, pa[k], desc_mnmajor(sV[bf], k), (j | k) != 0 ? 1u : 0u);
@@ -172,8 +243,10 @@ flash_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const float inv = (n_tiles > 0 && l > 0.f) ? 1.f / l : 0.f;
     const int row = rows[i];
-    if (row < row_limit) {
-      bf16* orow = p.o + (long long)(tok0 + row) * p.ldo + (long long)h * TC_D + q2;
+    bool keep = row < row_limit;
+    if constexpr (PAGED) keep = keep && row >= pg.q_start;   // zero-filled query rows before q_start are never stored
+    if (keep) {
+      bf16* orow = p.o + (long long)(tok0 + row - (PAGED ? pg.q_start : 0)) * p.ldo + (long long)h * TC_D + q2;
 #pragma unroll
       for (int t = 0; t < 16; ++t) {
         const float x0 = n_tiles > 0 ? o[4 * t + 2 * i] * inv : 0.f, x1 = n_tiles > 0 ? o[4 * t + 2 * i + 1] * inv : 0.f;
@@ -266,12 +339,18 @@ int launch_fwd_tc(const void* q, const void* k, const void* v, void* o, float* l
   static std::once_flag once;
   static cudaError_t err = cudaSuccess;
   std::call_once(once, [&] {
-    err = cudaFuncSetAttribute(flash_fwd_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM);
+    err = cudaFuncSetAttribute(flash_fwd_wgmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM);
   });
   MM_CHECK_CUDA(err);
-  flash_fwd_wgmma_kernel<<<grid, TC_THREADS, TC_SMEM, stream>>>(tq, tk, tv, p);
+  flash_fwd_wgmma_kernel<false><<<grid, TC_THREADS, TC_SMEM, stream>>>(tq, tk, tv, p, TcPagedParams{});
   MM_CHECK_LAUNCH();
   return MM_OK;
+}
+
+// log2 of a block size in [16, 256], or -1 (the block sizes of mm_decode_attn_paged)
+int paged_block_shift(int block_size) {
+  if (block_size < 16 || block_size > 256 || (block_size & (block_size - 1))) return -1;
+  return __builtin_ctz((unsigned)block_size);
 }
 
 }  // namespace
@@ -298,4 +377,50 @@ MM_API int mm_attn_fwd_tc_varlen(const void* q, const void* k, const void* v, vo
                "mm_attn_fwd_tc_varlen: segment tables missing");
   return launch_fwd_tc(q, k, v, o, lse, seg_len, seg_start, work, n_work, total_rows, ldq, ldk, ldv, ldo, n_seg, max_len,
                        Hq, Hkv, 1, scale, stream);
+}
+
+// Causal attention of query rows at positions q_start .. q_start + n_q - 1 of ONE sequence (q: [n_q, ldq]) over keys
+// and values 0 .. q_start + n_q - 1 in a paged pool (kpool / vpool [num_blocks, Hkv, block_size, 128], positions mapped
+// by block_table_row as in mm_decode_attn_paged). o: [n_q, ldo]. No lse.
+MM_API int mm_attn_fwd_tc_paged(const void* q, long long ldq, const void* kpool, const void* vpool, int num_blocks,
+                                const int* block_table_row, int max_blocks, int block_size, void* o, long long ldo,
+                                int q_start, int n_q, int Hq, int Hkv, int head_dim, float scale, cudaStream_t stream) {
+  const int shift = paged_block_shift(block_size);
+  MM_CHECK_ARG(shift >= 0, "mm_attn_fwd_tc_paged: block_size must be a power of two in [16,256] (got %d)", block_size);
+  MM_CHECK_ARG(max_blocks >= 1, "mm_attn_fwd_tc_paged: max_blocks must be >= 1 (got %d)", max_blocks);
+  MM_CHECK_ARG(block_table_row != nullptr, "mm_attn_fwd_tc_paged: block table missing");
+  MM_CHECK_ARG(head_dim == 128, "mm_attn_fwd_tc_paged: head_dim must be 128");
+  MM_CHECK_ARG(Hq > 0 && Hkv > 0 && Hq % Hkv == 0, "mm_attn_fwd_tc_paged: bad head counts");
+  MM_CHECK_ARG(num_blocks >= 1 && (long long)num_blocks * Hkv * block_size < (1ll << 31),
+               "mm_attn_fwd_tc_paged: num_blocks * Hkv * block_size must be in [1, 2^31)");
+  MM_CHECK_ARG(q_start >= 0 && n_q >= 1, "mm_attn_fwd_tc_paged: need q_start >= 0 and n_q >= 1 (got %d, %d)", q_start,
+               n_q);
+  MM_CHECK_ARG((long long)q_start + n_q <= (long long)max_blocks * block_size,
+               "mm_attn_fwd_tc_paged: q_start + n_q = %lld exceeds max_blocks * block_size = %lld",
+               (long long)q_start + n_q, (long long)max_blocks * block_size);
+  MM_CHECK_ARG(ldq % 8 == 0 && ldo % 8 == 0 && ((uintptr_t)q & 15) == 0 && ((uintptr_t)kpool & 15) == 0 &&
+                   ((uintptr_t)vpool & 15) == 0 && ((uintptr_t)o & 15) == 0,
+               "mm_attn_fwd_tc_paged: 16-byte alignment / pitch %% 8 required");
+  const int sb = block_size < TC_BC ? block_size : TC_BC;
+  const long long pool_rows = (long long)num_blocks * Hkv * block_size;
+  CUtensorMap tq, tk, tv;
+  int rc;
+  if ((rc = mm_attn_make_tmap_rows(&tq, q, (long long)Hq * 128, n_q, ldq))) return rc;
+  if ((rc = mm_attn_make_tmap_rows(&tk, kpool, 128, pool_rows, 128, sb))) return rc;
+  if ((rc = mm_attn_make_tmap_rows(&tv, vpool, 128, pool_rows, 128, sb))) return rc;
+  TcFwdParams p;
+  p.o = (bf16*)o; p.lse = nullptr; p.seqlens = nullptr; p.seg_start = nullptr; p.work = nullptr; p.ldo = ldo;
+  p.B = 1; p.T = q_start + n_q; p.Hq = Hq; p.Hkv = Hkv; p.scale = scale; p.causal = 1;
+  TcPagedParams pg;
+  pg.table = block_table_row; pg.q_start = q_start; pg.bs_shift = shift;
+  const int qt0 = q_start / TC_BR, qt1 = (q_start + n_q - 1) / TC_BR;
+  static std::once_flag once;
+  static cudaError_t err = cudaSuccess;
+  std::call_once(once, [&] {
+    err = cudaFuncSetAttribute(flash_fwd_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM);
+  });
+  MM_CHECK_CUDA(err);
+  flash_fwd_wgmma_kernel<true><<<dim3(qt1 - qt0 + 1, Hq, 1), TC_THREADS, TC_SMEM, stream>>>(tq, tk, tv, p, pg);
+  MM_CHECK_LAUNCH();
+  return MM_OK;
 }

@@ -110,6 +110,17 @@ class StackContext:
     x_final_in: Optional[torch.Tensor] = None  # input of the final norm
 
 
+@dataclass
+class PagedPrefill:
+    """One layer's view of a paged KV cache for a prefill that continues a cached prefix: the rows of `layer_forward`
+    are positions q_start .. q_start + T - 1 of ONE sequence, whose keys / values 0 .. q_start - 1 already sit in the
+    pool blocks named by `table_row`. q_start is a multiple of the block size."""
+    kpool: torch.Tensor          # [num_blocks, Hkv, block_size, dh] of this layer
+    vpool: torch.Tensor
+    table_row: torch.Tensor      # int32 [max_blocks] (device)
+    q_start: int
+
+
 class LlamaStack:
     """Forward/backward over a list of LayerWeights. Stateless apart from the RoPE tables."""
 
@@ -126,7 +137,9 @@ class LlamaStack:
 
     # ------------------------------------------------------------------ forward
     def layer_forward(self, w: LayerWeights, x: torch.Tensor, ctx: StackContext, save: bool,
-                      save_gu: bool) -> torch.Tensor:
+                      save_gu: bool, paged: Optional[PagedPrefill] = None) -> torch.Tensor:
+        """paged: the rows continue a sequence cached in a paged pool (prefix caching). Their post-RoPE K/V are written
+        into the pool blocks from position q_start on, and attention reads keys 0 .. q_start + T - 1 from the pool."""
         d = self.dims
         B, T = ctx.B, ctx.T
         Hq, Hkv, dh = d.n_heads, d.n_kv_heads, d.head_dim
@@ -135,7 +148,14 @@ class LlamaStack:
         del n1
         ops.rope_(qkv, ctx.pos, self.cos, self.sin, Hq + Hkv, dh)
         q, k, v = qkv[:, :Hq * dh], qkv[:, Hq * dh:(Hq + Hkv) * dh], qkv[:, (Hq + Hkv) * dh:]
-        if ctx.segments is None:
+        if paged is not None:
+            bs = paged.kpool.shape[2]
+            assert B == 1 and paged.q_start % bs == 0, "a paged prefill continues one sequence at a block boundary"
+            ops.kv_prefill_paged(qkv, paged.kpool, paged.vpool, paged.table_row[paged.q_start // bs:], x.shape[0], Hq,
+                                 Hkv, dh)
+            attn, lse = ops.attn_fwd_paged(q, paged.kpool, paged.vpool, paged.table_row, paged.q_start, Hq, Hkv, dh,
+                                           self.scale), None
+        elif ctx.segments is None:
             attn, lse = ops.attn_fwd(q, k, v, B, T, Hq, Hkv, dh, True, self.scale, seqlens=ctx.seqlens,
                                      need_lse=save)
         else:

@@ -19,6 +19,10 @@ With `kv_pool_tokens` set, the slots share a paged KV cache instead of each rese
 of fixed-size blocks per layer and a device block table [max_slots, ceil(max_context / kv_block_size)] (see
 KVBlockAllocator for the reservation and reclaim rules). The paged attention kernel gives the dense one's bits, so a
 request's output does not depend on the cache layout or on which blocks it received.
+A paged server also caches prompt prefixes: `h = cache_prefix(prefix)` prefills the prefix's whole blocks once,
+`submit(suffix, prefix=h)` shares them and prefills only the prefix tail and the suffix (attention reads the shared
+keys through the block table, `ops.attn_fwd_paged`), and `drop_prefix(h)` lets the blocks go once no request uses them.
+The request returns the bits of the whole prompt submitted without a prefix.
 Every request's output equals what `greedy_decode` produces for it alone (tests/test_decode_gpu.py), a forced schedule
 shorter than the run included: in both, the request free-runs once its schedule ends (tests/test_serve_lifecycle_gpu.py).
 """
@@ -34,17 +38,30 @@ from .. import ops
 from ..constants import EOS_TOKEN_IDS, IMAGE_END_TOKEN_ID, IMAGE_START_TOKEN_ID
 from .decode import check_forced_tokens
 from .decode_step import decode_heads, decoder_stack_step
-from .llama import StackContext
+from .llama import PagedPrefill, StackContext
 from .sampling import SamplingArrays, SamplingParams
+
+
+class PrefixHandle:
+    """A prompt prefix cached by one paged `ContinuousBatcher` (`cache_prefix`). Its first `shared_len` positions (whole
+    KV blocks) are prefilled once and shared by every request submitted with `prefix=` this handle; the `length -
+    shared_len` tail rows are kept as embeddings and prefilled with each request's suffix."""
+
+    def __init__(self, server, pid: int, length: int, shared_len: int, tail: torch.Tensor):
+        self.server, self.pid, self.length, self.shared_len, self.tail = server, pid, length, shared_len, tail
+
+    def __repr__(self):
+        return f"PrefixHandle(pid={self.pid}, length={self.length}, shared_len={self.shared_len})"
 
 
 @dataclass
 class _Request:
     rid: int
-    embeds: torch.Tensor                 # [P, H] bf16 (device)
+    embeds: torch.Tensor                 # [P - start, H] bf16 (device): the prompt rows from position `start` on
     max_new_tokens: int
     forced: Optional[torch.Tensor]       # [n] int32 (host) or None
     sampling: Optional[SamplingParams] = None
+    prefix: Optional[PrefixHandle] = None   # positions 0 .. start-1 are this prefix's shared blocks (start = shared_len)
     slot: int = -1
     sent_ids: int = 0
     sent_img: int = 0
@@ -63,7 +80,12 @@ class KVBlockAllocator:
     max_new_tokens n, the prefill writes positions 0 .. P-2 and the decode state machine (decode_state_kernel) feeds
     the token at pos-1, starting at pos = P and advancing pos once per step for at most n+1 steps; a finished slot
     keeps rewriting its frozen position pos-1 = P+n until the host reclaims it. So positions 0 .. P+n are written and
-    read: ceil((P + n + 1) / block_size) blocks, never more (an early EOS only freezes the slot sooner)."""
+    read: ceil((P + n + 1) / block_size) blocks, never more (an early EOS only freezes the slot sooner).
+
+    Shared prefix blocks: `pin` takes the blocks of a cached prefix, held by the prefix handle and by every queued and
+    running request that names it (`ref`); they return to the free list when the last of these lets go. A request on a
+    prefix of Ls positions (a multiple of block_size) reserves only its private blocks, reservation(P - Ls, n): positions
+    Ls .. P+n, the only ones it writes."""
 
     def __init__(self, num_blocks: int, block_size: int):
         check_kv_block_size(block_size)
@@ -73,6 +95,9 @@ class KVBlockAllocator:
         self.scratch = num_blocks
         self.free: List[int] = list(range(num_blocks))   # handed out from the front, returned to the back
         self.owned: Dict[int, List[int]] = {}
+        self.shared: Dict[int, List[int]] = {}           # prefix id -> its pinned blocks
+        self.refs: Dict[int, int] = {}                   # prefix id -> holders (the handle, queued and running requests)
+        self.prefix_of: Dict[int, int] = {}              # request id -> the prefix it names
 
     def reservation(self, prompt_len: int, max_new_tokens: int) -> int:
         """Blocks a request of `prompt_len` positions and `max_new_tokens` new tokens holds while it runs."""
@@ -89,7 +114,34 @@ class KVBlockAllocator:
         return blocks
 
     def release(self, rid: int) -> None:
+        """A request is handed out: its private blocks go back, and its hold on a shared prefix ends."""
         self.free.extend(self.owned.pop(rid))
+        if rid in self.prefix_of:
+            self.unref(self.prefix_of.pop(rid))
+
+    def pinned(self) -> int:
+        """Blocks held by cached prefixes (dropped ones included until their last user is handed out)."""
+        return sum(len(b) for b in self.shared.values())
+
+    def pin(self, pid: int, n_blocks: int) -> List[int]:
+        """Take n_blocks for prefix `pid`, held by its handle."""
+        assert pid not in self.shared, f"prefix {pid} already holds blocks"
+        assert self.can_reserve(n_blocks), f"{n_blocks} blocks requested, {len(self.free)} free"
+        blocks, self.free = self.free[:n_blocks], self.free[n_blocks:]
+        self.shared[pid], self.refs[pid] = blocks, 1
+        return blocks
+
+    def ref(self, pid: int, rid: int) -> None:
+        """Request `rid` names prefix `pid` from submission until it is handed out (release)."""
+        assert pid in self.shared and rid not in self.prefix_of
+        self.refs[pid] += 1
+        self.prefix_of[rid] = pid
+
+    def unref(self, pid: int) -> None:
+        self.refs[pid] -= 1
+        if self.refs[pid] == 0:
+            del self.refs[pid]
+            self.free.extend(self.shared.pop(pid))
 
 
 def check_kv_block_size(block_size) -> None:
@@ -159,6 +211,8 @@ class ContinuousBatcher:
         self.queue: Deque[_Request] = deque()
         self.slots: List[Optional[_Request]] = [None] * B
         self.next_rid = 0
+        self.prefixes: Dict[int, PrefixHandle] = {}    # cached prefixes not yet dropped
+        self.next_pid = 0
         self.steps_run = 0
         self.samp = SamplingArrays(B, dev)
         self.graph = None                  # greedy step
@@ -211,44 +265,132 @@ class ContinuousBatcher:
     # ------------------------------------------------------------------ requests
     @torch.no_grad()
     def submit(self, inputs_embeds: torch.Tensor, max_new_tokens: Optional[int] = None,
-               forced_tokens: Optional[torch.Tensor] = None, sampling: Optional[SamplingParams] = None) -> int:
+               forced_tokens: Optional[torch.Tensor] = None, sampling: Optional[SamplingParams] = None,
+               prefix: Optional[PrefixHandle] = None) -> int:
         """inputs_embeds: [P, H] or [1, P, H] prompt embeddings (text + projected image rows, as `generate` builds
         them). sampling: None or temperature 0 = greedy; otherwise the request draws its tokens with these parameters
         and seed, and its output is the same whatever other requests share the server. forced_tokens: integer ids
         indexed by the request's step count; an entry >= 0 replaces the step's token, -1 and every step past the
         schedule's end are free-running (as in `DecodeEngine.generate`). Ids outside [-1, embedding rows) raise
         ValueError here, before any device work, and so does a request whose KV blocks exceed a paged server's whole
-        pool. Returns the request id."""
+        pool. prefix: a handle from this server's `cache_prefix`; the prompt is then the prefix followed by
+        inputs_embeds (the suffix, at least one row), and the request returns exactly what that whole prompt submitted
+        without a prefix returns. Returns the request id."""
         check_forced_tokens(forced_tokens, self.inner.embed_tokens.weight.shape[0])
         if sampling is not None and not isinstance(sampling, SamplingParams):
             raise ValueError("sampling must be a SamplingParams or None")
+        if prefix is not None:
+            self._check_handle(prefix)
         P = inputs_embeds.reshape(-1, inputs_embeds.shape[-1]).shape[0]
         n_new = self.cap if max_new_tokens is None else int(max_new_tokens)
         if n_new > self.cap:
             raise ValueError(f"max_new_tokens {n_new} exceeds the server's limit {self.cap}")
+        if prefix is not None:
+            if P < 1:
+                raise ValueError("a request on a cached prefix needs a suffix of at least one row")
+            P += prefix.length
         if P < 1 or P + n_new + 2 > self.Tmax:
             raise ValueError(f"prompt of {P} positions + {n_new} new ones does not fit max_context {self.Tmax}")
-        if self.alloc is not None and self.alloc.reservation(P, n_new) > self.alloc.num_blocks:
-            raise ValueError(f"prompt of {P} positions + {n_new} new ones needs {self.alloc.reservation(P, n_new)} "
-                             f"KV blocks, more than the whole pool of {self.alloc.num_blocks}")
+        if self.alloc is not None:
+            start = prefix.shared_len if prefix is not None else 0
+            need, avail = self.alloc.reservation(P - start, n_new), self.alloc.num_blocks - self.alloc.pinned()
+            if need > avail:
+                where = (f"the whole pool of {avail}" if avail == self.alloc.num_blocks else
+                         f"the {avail} blocks of the pool outside its cached prefixes")
+                raise ValueError(f"prompt of {P} positions + {n_new} new ones needs {need} KV blocks, more than {where}")
         e = inputs_embeds.reshape(-1, inputs_embeds.shape[-1]).to(self.dev, dtype=torch.bfloat16).contiguous()
+        if prefix is not None:
+            e = torch.cat([prefix.tail, e])
         f = None if forced_tokens is None else forced_tokens.reshape(-1).to(torch.int32).cpu()
         rid = self.next_rid
         self.next_rid += 1
-        self.queue.append(_Request(rid, e, n_new, f, sampling if sampling is not None and not sampling.greedy else None))
+        if prefix is not None:
+            self.alloc.ref(prefix.pid, rid)
+        self.queue.append(_Request(rid, e, n_new, f, sampling if sampling is not None and not sampling.greedy else None,
+                                   prefix=prefix))
         return rid
+
+    # ------------------------------------------------------------------ cached prefixes
+    def _check_handle(self, h) -> None:
+        if self.alloc is None:
+            raise ValueError("prefix caching needs a paged server (kv_pool_tokens)")
+        if not isinstance(h, PrefixHandle) or h.server is not self or self.prefixes.get(h.pid) is not h:
+            raise ValueError(f"{h!r} is not a live prefix of this server (unknown, dropped or another server's)")
+
+    @torch.no_grad()
+    def cache_prefix(self, prefix_embeds: torch.Tensor) -> PrefixHandle:
+        """Prefill a prompt prefix ([Lp, H] or [1, Lp, H]) once and keep its KV blocks for `submit(..., prefix=h)`.
+        The first Ls = floor(Lp / block_size) * block_size positions are prefilled now into Ls / block_size pinned
+        blocks, which requests on the prefix share and never write; the remaining Lp - Ls rows are kept as embeddings
+        and prefilled with each request's suffix. Paged servers only. Raises ValueError, before any device work, for a
+        prefix shorter than one block, one that leaves no room for a request in max_context, and one whose blocks are
+        not free now or would leave a queued request more private blocks than the pool holds outside the prefixes."""
+        if self.alloc is None:
+            raise ValueError("prefix caching needs a paged server (kv_pool_tokens)")
+        bs = self.alloc.block_size
+        Lp = prefix_embeds.reshape(-1, prefix_embeds.shape[-1]).shape[0]
+        Ls = Lp // bs * bs
+        if Ls == 0:
+            raise ValueError(f"a prefix of {Lp} positions is shorter than one KV block ({bs}) and shares nothing")
+        if Lp + 3 > self.Tmax:
+            raise ValueError(f"a prefix of {Lp} positions leaves no room for a request in max_context {self.Tmax}")
+        n_sh = Ls // bs
+        if not self.alloc.can_reserve(n_sh):
+            raise ValueError(f"the prefix needs {n_sh} KV blocks and only {len(self.alloc.free)} are free now")
+        avail = self.alloc.num_blocks - self.alloc.pinned() - n_sh
+        worst = max((self.alloc.reservation(r.embeds.shape[0], r.max_new_tokens) for r in self.queue), default=0)
+        if worst > avail:
+            raise ValueError(f"pinning {n_sh} blocks would leave {avail} for requests, and a queued request needs {worst}")
+        d = self.d
+        Hq, Hkv, dh = d.n_heads, d.n_kv_heads, d.head_dim
+        e = prefix_embeds.reshape(-1, prefix_embeds.shape[-1]).to(self.dev, dtype=torch.bfloat16).contiguous()
+        pid = self.next_pid
+        self.next_pid += 1
+        blocks = self.alloc.pin(pid, n_sh)
+        row = torch.tensor(blocks, dtype=torch.int32).to(self.dev)
+        ctx = StackContext(B=1, T=Ls, pos=torch.arange(Ls, dtype=torch.int32, device=self.dev), seqlens=None)
+        x = e[:Ls]
+        for i, w in enumerate(self.layers):
+            x = self.stack.layer_forward(w, x, ctx, save=True, save_gu=False)
+            s = ctx.saved.pop()
+            ops.kv_prefill_paged(s.qkv, self.kc[i], self.vc[i], row, Ls, Hq, Hkv, dh)
+            del s
+        h = PrefixHandle(self, pid, Lp, Ls, e[Ls:].clone())
+        self.prefixes[pid] = h
+        return h
+
+    def drop_prefix(self, h: PrefixHandle) -> None:
+        """Forget a cached prefix: no new request may name it, and its blocks return to the pool once no queued or
+        running request uses it."""
+        self._check_handle(h)
+        del self.prefixes[h.pid]
+        self.alloc.unref(h.pid)
 
     @torch.no_grad()
     def _admit(self, req: _Request, b: int):
         d = self.d
         Hq, Hkv, dh = d.n_heads, d.n_kv_heads, d.head_dim
-        P = req.embeds.shape[0]
-        if self.alloc is not None:  # the slot's table row: its reserved blocks, then scratch
+        P = req.embeds.shape[0]                        # prompt rows held: P - Ls on a prefix of Ls shared positions
+        if self.alloc is not None:  # the slot's table row: [its prefix's shared blocks,] its reserved blocks, then scratch
             blocks = self.alloc.reserve(req.rid, self.alloc.reservation(P, req.max_new_tokens))
+            if req.prefix is not None:
+                blocks = self.alloc.shared[req.prefix.pid] + blocks
             row = torch.full((self.max_blocks,), self.alloc.scratch, dtype=torch.int32)
             row[:len(blocks)] = torch.tensor(blocks, dtype=torch.int32)
             self.table[b].copy_(row.to(self.dev, non_blocking=True))
-        if P > 1:   # prefill positions 0..P-2 into the slot's cache region
+        if req.prefix is not None:
+            # positions Ls .. Ls+P-2 (prefix tail + suffix but its last row) continue the shared blocks; every layer
+            # writes their K/V into the private blocks and attends through the pool
+            Ls = req.prefix.shared_len
+            if P > 1:
+                pos = torch.arange(Ls, Ls + P - 1, dtype=torch.int32, device=self.dev)
+                ctx = StackContext(B=1, T=P - 1, pos=pos, seqlens=None)
+                x = req.embeds[:P - 1].contiguous()
+                for i, w in enumerate(self.layers):
+                    x = self.stack.layer_forward(w, x, ctx, save=False, save_gu=False,
+                                                 paged=PagedPrefill(self.kc[i], self.vc[i], self.table[b], Ls))
+            P += Ls
+        elif P > 1:   # prefill positions 0..P-2 into the slot's cache region
             pos = torch.arange(P - 1, dtype=torch.int32, device=self.dev)
             ctx = StackContext(B=1, T=P - 1, pos=pos, seqlens=None)
             x = req.embeds[:P - 1].contiguous()
@@ -260,7 +402,7 @@ class ContinuousBatcher:
                 else:
                     ops.kv_prefill_paged(s.qkv, self.kc[i], self.vc[i], self.table[b], P - 1, Hq, Hkv, dh)
                 del s
-        self.xin[b].copy_(req.embeds[P - 1])
+        self.xin[b].copy_(req.embeds[-1])             # the last prompt row, fed at position P-1
         row = torch.full((self.forced.shape[1],), -1, dtype=torch.int32)
         if req.forced is not None:
             n = min(row.numel(), req.forced.numel())
@@ -282,7 +424,7 @@ class ContinuousBatcher:
             return None
         b = next((i for i, s in enumerate(self.slots) if s is None), None)
         if b is not None and self.alloc is not None:
-            head = self.queue[0]
+            head = self.queue[0]                   # (on a prefix, the rows held give its private blocks alone)
             if not self.alloc.can_reserve(self.alloc.reservation(head.embeds.shape[0], head.max_new_tokens)):
                 return None
         return b

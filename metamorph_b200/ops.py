@@ -516,6 +516,24 @@ def kv_prefill_paged(qkv, kpool, vpool, table_row, T, Hq, Hkv, head_dim):
          stream_ptr())
 
 
+def attn_fwd_paged(q, kpool, vpool, table_row, q_start, Hq, Hkv, head_dim, scale, out=None):
+    """Causal attention of the query rows of positions q_start .. q_start + n_q - 1 (q: [n_q, *] row-major view, e.g. the
+    Q columns of a fused qkv) over keys / values 0 .. q_start + n_q - 1 of a paged pool (kpool / vpool [num_blocks, Hkv,
+    block_size, head_dim], table_row [max_blocks] int32 on the device). Row r of the output is bit-identical to row r of
+    attn_fwd(B=1, T=q_start + n_q, causal) on the same K/V. Returns out [n_q, Hq * head_dim]."""
+    require_cuda(q, kpool, vpool, table_row, out)
+    assert q.dim() == 2 and q.stride(1) == 1
+    assert kpool.dim() == 4 and kpool.is_contiguous() and vpool.shape == kpool.shape and vpool.is_contiguous()
+    assert table_row.dtype == torch.int32 and table_row.dim() == 1 and table_row.stride(0) == 1
+    n_q = q.shape[0]
+    if out is None:
+        out = torch.empty((n_q, Hq * head_dim), dtype=torch.bfloat16, device=q.device)
+    call("mm_attn_fwd_tc_paged", ptr(q), ll(q.stride(0)), ptr(kpool), ptr(vpool), c_int(kpool.shape[0]), ptr(table_row),
+         c_int(table_row.shape[0]), c_int(kpool.shape[2]), ptr(out), ll(out.stride(0)), c_int(q_start), c_int(n_q),
+         c_int(Hq), c_int(Hkv), c_int(head_dim), c_float(scale), stream_ptr())
+    return out
+
+
 def decode_state_step(st: dict, argmax_tok, forced, step, B, num_image_tokens, max_new_tokens,
                       start_id, end_id, eos0, eos1, pred_z, img_out):
     call("mm_decode_state_step", ptr(st["in_image_mode"]), ptr(st["total_image_tokens"]),
