@@ -101,6 +101,22 @@ int mm_argmax_rows(const float* logits, long long ld, long long R, int V, int* o
  * -inf). Every per-row array is a device pointer. One launch of R thread-block clusters of 8 CTAs; V <= 393216. */
 int mm_sample_rows(const float* logits, long long ld, long long R, int V, const float* temperature, const int* top_k,
                    const float* top_p, const unsigned long long* seed, const int* counter, int* out, cudaStream_t s);
+/* Log-probabilities of the tokens a decode step emitted, read after mm_decode_state_step[_slots]: for the model's raw
+ * distribution over one fp32 logits row (NaN read as -inf, m = max l, S = sum_j exp(l_j - m)),
+ * logprob(i) = l_i - m - ln S, rounded once to fp32 from an fp64 evaluation (S summed in fp64 from expf terms; within
+ * 0.5 ulp + 2^-21 + 2^-51 |logprob| of the exact value). A row whose max is +inf is the point mass on its c +inf
+ * entries (-ln c each, -inf elsewhere); a row with no logit above -inf reports NaN. Row r reports when
+ * append_kind[r] == 0 (the step appended next_token = token[r] to ids_out), n_top[r] >= 0 (-1: skip) and
+ * 0 <= n_ids[r] - 1 < max_ids; it then writes slot o = r * max_ids + n_ids[r] - 1 and nothing else:
+ * lp_out[o] = logprob(token[r]) (NaN for a token outside [0, V)), and for k < min(n_top[r], 20)
+ * top_ids[o * 20 + k], top_lp[o * 20 + k] = the k-th entry in order of logit descending, lowest index first among
+ * ties (mm_argmax_rows' order); entries past V get id -1 and logprob -inf. The bits are a pure function of the row's
+ * logits and V, and a token in the list has the same bits there as in lp_out. lp_out [R, max_ids],
+ * top_ids / top_lp [R, max_ids, 20]; every pointer is a device pointer. One launch of R clusters of 8 CTAs;
+ * V <= 393216. */
+int mm_decode_logprobs(const float* logits, long long ld, long long R, int V, const int* append_kind, const int* token,
+                       const int* n_ids, const int* n_top, int max_ids, float* lp_out, int* top_ids, float* top_lp,
+                       cudaStream_t s);
 
 /* torch.optim.AdamW step (train.py:82 --optim adamw_torch), fused over flat buffers; clip coefficient. */
 int mm_adamw_step(void* p16, float* p32, float* m, float* v, const void* grad, int grad_f32, long long n, float lr,

@@ -284,6 +284,177 @@ sample_rows_kernel(const float* __restrict__ logits, long long ld, int V, int S,
   cluster.sync();
 }
 
+// ---------------------------------------------------------------- log-probabilities of the emitted token
+// logprob(i) = l_i - m - ln S over the raw logits (NaN read as -inf), m = max l, S = sum_j exp(l_j - m), rounded once to
+// fp32. Each term is expf(d_hi) * (1 + d_lo) with d = l_j - m split into fp32 d_hi and the fp64 remainder d_lo, so the
+// term carries expf's 2 ulp and nothing of the fp32 rounding of d; S is summed in fp64 in a fixed order (per thread
+// j = tid, tid + 512, ..., the warp tree, warps in order, CTAs in rank order) that depends on V alone.
+// The top-n list orders (l, index) by value descending, lowest index first among ties: mm_argmax_rows' order.
+constexpr int kTopMax = 20;
+
+struct LogprobShared {
+  float sval[kSampleThreads / 32];
+  int sidx[kSampleThreads / 32];
+  float wmax[kSampleThreads / 32];
+  int wcnt[kSampleThreads / 32];
+  double wsum[kSampleThreads / 32];
+  float cmax;                           // this CTA's partials for the cluster: max, count of +inf, sum of exp(l - m)
+  int ccnt;
+  double csum;
+  float top_v[kTopMax];                 // this CTA's top-n, in order; index 0x7fffffff = no entry
+  int top_i[kTopMax];
+  float pick_v;
+  int pick_i;
+  float row_max;
+};
+
+// (v, i) comes strictly after (pv, pi) in the top-n order
+__device__ __forceinline__ bool after(float v, int i, float pv, int pi) { return v < pv || (v == pv && i > pi); }
+
+// mode 0: a distribution (lnS = ln S); 1: max is +inf (lnS = ln c, c = count of +inf); 2: no logit above -inf
+__device__ __forceinline__ float logprob_of(float v, float m, double lnS, int mode) {
+  if (mode == 2) return __int_as_float(0x7fffffff);
+  if (mode == 1) return v == INFINITY ? (float)(-lnS) : -INFINITY;
+  return (float)(((double)v - (double)m) - lnS);
+}
+
+__global__ void __cluster_dims__(kSampleCTAs, 1, 1) __launch_bounds__(kSampleThreads, 1)
+decode_logprobs_kernel(const float* __restrict__ logits, long long ld, int V, int S,
+                       const int* __restrict__ append_kind, const int* __restrict__ token,
+                       const int* __restrict__ n_ids, const int* __restrict__ n_top, int max_ids,
+                       float* __restrict__ lp_out, int* __restrict__ top_ids, float* __restrict__ top_lp) {
+  extern __shared__ __align__(16) unsigned char dyn[];
+  __shared__ LogprobShared sh;
+  float* zs = reinterpret_cast<float*>(dyn);
+  cg::cluster_group cluster = cg::this_cluster();
+  const int rank = (int)cluster.block_rank(), tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const long long r = blockIdx.x / kSampleCTAs;
+  // every CTA of the cluster reads the same gate, so a skipped row leaves without touching the cluster
+  const int slot = n_ids[r] - 1, nt = n_top[r];
+  if (append_kind[r] != 0 || nt < 0 || slot < 0 || slot >= max_ids) return;
+  const int ntop = min(nt, kTopMax);
+  const int j0 = rank * S;
+  const int n = max(0, min(S, V - j0));
+  const float* x = logits + r * ld + j0;
+
+  // load the slice (NaN -> -inf); the thread's first entry in the top-n order, its max and its count of +inf
+  float cv = -INFINITY;
+  int ci = 0x7fffffff, cnt = 0;
+  for (int j = tid; j < n; j += kSampleThreads) {
+    float v = x[j];
+    if (isnan(v)) v = -INFINITY;
+    zs[j] = v;
+    better(cv, ci, v, j0 + j);
+    cnt += v == INFINITY;
+  }
+  float mx = cv;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  }
+  if (lane == 0) { sh.wmax[warp] = mx; sh.wcnt[warp] = cnt; }
+  __syncthreads();
+  if (tid == 0) {
+    for (int w = 1; w < kSampleThreads / 32; ++w) { mx = fmaxf(mx, sh.wmax[w]); cnt += sh.wcnt[w]; }
+    sh.cmax = mx;
+    sh.ccnt = cnt;
+  }
+  cluster.sync();                                        // every CTA's max and count are published
+  if (tid == 0) {
+    float m = -INFINITY;
+    for (int q = 0; q < kSampleCTAs; ++q) m = fmaxf(m, cluster.map_shared_rank(&sh, q)->cmax);
+    sh.row_max = m;
+  }
+  __syncthreads();
+  const float m = sh.row_max;
+
+  // S over the slice, fp64 (only a finite max has terms; the special rows need none)
+  double s = 0.0;
+  if (m > -INFINITY && m < INFINITY) {
+    for (int j = tid; j < n; j += kSampleThreads) {
+      const double d = (double)zs[j] - (double)m;        // -inf for a -inf logit
+      if (d > -110.0) {                                  // below, expf(d) < 2^-158: the term rounds to 0
+        const float dh = (float)d;
+        s += (double)expf(dh) * (1.0 + (d - (double)dh));
+      }
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) sh.wsum[warp] = s;
+
+  // this CTA's top-n: each thread holds its first entry after the last pick; only the pick's owner looks further
+  for (int k = 0; k < ntop; ++k) {
+    float bv = cv;
+    int bj = ci;
+    block_argmax(bv, bj, sh.sval, sh.sidx);
+    if (tid == 0) { sh.top_v[k] = bv; sh.top_i[k] = bj; sh.pick_v = bv; sh.pick_i = bj; }
+    __syncthreads();
+    const float pv = sh.pick_v;
+    const int pi = sh.pick_i;
+    if (pi != 0x7fffffff && ci == pi) {
+      cv = -INFINITY;
+      ci = 0x7fffffff;
+      for (int j = tid; j < n; j += kSampleThreads)
+        if (after(zs[j], j0 + j, pv, pi)) better(cv, ci, zs[j], j0 + j);
+    }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    s = 0.0;
+    for (int w = 0; w < kSampleThreads / 32; ++w) s += sh.wsum[w];
+    sh.csum = s;
+  }
+  cluster.sync();                                        // every CTA's sum and top-n are published
+
+  if (rank == 0 && tid == 0) {
+    int mode = 0, c = 0;
+    double sum = 0.0;
+    for (int q = 0; q < kSampleCTAs; ++q) {
+      const LogprobShared* o = cluster.map_shared_rank(&sh, q);
+      sum += o->csum;
+      c += o->ccnt;
+    }
+    double lnS = 0.0;
+    if (!(m > -INFINITY)) mode = 2;
+    else if (m == INFINITY) { mode = 1; lnS = log((double)c); }
+    else lnS = log(sum);
+    const long long o = r * max_ids + slot;
+    const int t = token[r];
+    float vt = __int_as_float(0x7fffffff);               // a token outside [0, V) reports NaN
+    if (t >= 0 && t < V) {
+      vt = logits[r * ld + t];
+      vt = logprob_of(isnan(vt) ? -INFINITY : vt, m, lnS, mode);
+    }
+    lp_out[o] = vt;
+    // merge the CTAs' sorted lists: each step takes the first head in the order
+    int head[kSampleCTAs];
+#pragma unroll
+    for (int q = 0; q < kSampleCTAs; ++q) head[q] = 0;
+    for (int k = 0; k < ntop; ++k) {
+      float bv = -INFINITY;
+      int bj = 0x7fffffff, bq = -1;
+#pragma unroll
+      for (int q = 0; q < kSampleCTAs; ++q) {
+        const LogprobShared* p = cluster.map_shared_rank(&sh, q);
+        if (head[q] < ntop && p->top_i[head[q]] != 0x7fffffff) {
+          const float v = p->top_v[head[q]];
+          const int i = p->top_i[head[q]];
+          if (v > bv || (v == bv && i < bj)) { bv = v; bj = i; bq = q; }
+        }
+      }
+      if (bq >= 0) {
+#pragma unroll
+        for (int q = 0; q < kSampleCTAs; ++q) head[q] += q == bq;
+      }
+      top_ids[o * kTopMax + k] = bq >= 0 ? bj : -1;      // fewer than n entries (V < n): id -1, logprob -inf
+      top_lp[o * kTopMax + k] = bq >= 0 ? logprob_of(bv, m, lnS, mode) : -INFINITY;
+    }
+  }
+  cluster.sync();                                        // keep every CTA's shared memory alive for rank 0
+}
+
 }  // namespace
 
 MM_API int mm_sample_rows(const float* logits, long long ld, long long R, int V, const float* temperature,
@@ -305,6 +476,30 @@ MM_API int mm_sample_rows(const float* logits, long long ld, long long R, int V,
   MM_CHECK_CUDA(attr_err);
   sample_rows_kernel<<<(unsigned)(R * kSampleCTAs), kSampleThreads, smem_bytes(S), stream>>>(
       logits, ld, V, S, temperature, top_k, top_p, seed, counter, out);
+  MM_CHECK_LAUNCH();
+  return MM_OK;
+}
+
+MM_API int mm_decode_logprobs(const float* logits, long long ld, long long R, int V, const int* append_kind,
+                              const int* token, const int* n_ids, const int* n_top, int max_ids, float* lp_out,
+                              int* top_ids, float* top_lp, cudaStream_t stream) {
+  MM_CHECK_ARG(R > 0 && V > 0 && ld >= V && max_ids > 0,
+               "mm_decode_logprobs: bad shape (need R>0, V>0, ld>=V, max_ids>0)");
+  MM_CHECK_ARG(R <= 0x7fffffffll / kSampleCTAs, "mm_decode_logprobs: too many rows");
+  const int S = ((V + kSampleCTAs - 1) / kSampleCTAs + 3) / 4 * 4;   // the slice rule of mm_sample_rows
+  MM_CHECK_ARG(S <= kMaxSlice, "mm_decode_logprobs: V=%d exceeds the shared-memory budget (V <= %d)", V,
+               kSampleCTAs * kMaxSlice);
+  MM_CHECK_ARG(logits && append_kind && token && n_ids && n_top && lp_out && top_ids && top_lp,
+               "mm_decode_logprobs: null pointer");
+  static std::once_flag once;
+  static cudaError_t attr_err = cudaSuccess;
+  std::call_once(once, [] {
+    attr_err = cudaFuncSetAttribute(decode_logprobs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    kMaxSlice * 4);
+  });
+  MM_CHECK_CUDA(attr_err);
+  decode_logprobs_kernel<<<(unsigned)(R * kSampleCTAs), kSampleThreads, (size_t)S * 4, stream>>>(
+      logits, ld, V, S, append_kind, token, n_ids, n_top, max_ids, lp_out, top_ids, top_lp);
   MM_CHECK_LAUNCH();
   return MM_OK;
 }

@@ -16,6 +16,7 @@ from .. import ops
 from ..constants import EOS_TOKEN_IDS, IMAGE_END_TOKEN_ID, IMAGE_START_TOKEN_ID
 from .decode_step import decode_heads, decoder_stack_step
 from .llama import StackContext
+from .logprobs import LogprobBuffers, check_logprobs
 from .sampling import SamplingArrays, SamplingParams, per_sequence
 
 
@@ -44,7 +45,8 @@ class DecodeEngine:
                  end_image_token_id: int = IMAGE_END_TOKEN_ID, eos_token_id=EOS_TOKEN_IDS,
                  forced_tokens: Optional[torch.Tensor] = None, poll_every: int = 16,
                  max_steps: Optional[int] = None,
-                 sampling: Union[None, SamplingParams, Sequence[SamplingParams]] = None):
+                 sampling: Union[None, SamplingParams, Sequence[SamplingParams]] = None,
+                 logprobs: Optional[int] = None):
         """inputs_embeds [B, P, H] (right-padded to P; prompt_lens[b] valid rows). B <= 128.
         sampling: None (greedy), one SamplingParams (sequence b draws with seed + b) or one per sequence. The draw
         replaces the argmax only: image mode, the EOS test on the drawn token and forced tokens are unchanged. When
@@ -53,7 +55,12 @@ class DecodeEngine:
         step's token, -1 is free-running, and so is every step past column n - 1: a schedule shorter than the run ends
         and the sequence free-runs from there, exactly as a request served by `ContinuousBatcher` does. Ids outside
         [-1, embedding rows) raise ValueError before any device work.
-        Returns (ids list per sequence (int32 tensors), image_embeds list per sequence [n, C])."""
+        logprobs: None, or an int n in [0, 20]: every sequence also reports, for each id it emits, that id's
+        log-probability under the step's raw distribution and the n most likely ids with theirs (engine/logprobs.py).
+        Anything else raises ValueError before any device work. Ids and embeddings do not change.
+        Returns (ids list per sequence (int32 tensors), image_embeds list per sequence [n, C]), and with logprobs a
+        third element: one TokenLogprobs per sequence, entry k belonging to ids[k]."""
+        check_logprobs(logprobs)
         B, P, H = inputs_embeds.shape
         assert B <= 128, f"decode batch is limited to 128 sequences per step (got {B}): the weight-streaming GEMM " \
                          "serves at most 128 batch rows"
@@ -112,12 +119,18 @@ class DecodeEngine:
         xin = torch.empty((B, H), dtype=torch.bfloat16, device=dev)
         V = m.lm_head.weight.shape[0]
         logits = torch.empty((B, (V + 7) // 8 * 8), dtype=torch.float32, device=dev)
+        lpb = None
+        if logprobs is not None:
+            lpb = LogprobBuffers(B, st["ids_out"].shape[1], dev)
+            lpb.n_top.fill_(int(logprobs))
 
         def heads_and_state(h_pre_norm, step):
             tok, pred_z, prediction = decode_heads(m, h_pre_norm, st["in_image_mode"], logits, V, samp,
                                                    st["total_output"])
             ops.decode_state_step(st, tok, forced, step, B, ntok, max_new_tokens, start_image_token_id,
                                   end_image_token_id, eos0, eos1, pred_z, img_out)
+            if lpb is not None:
+                lpb.launch(logits, V, st)
             ops.decode_next_input(st["append_kind"], st["next_token"], model.embed_tokens.weight.data,
                                   prediction, xin)
 
@@ -169,4 +182,6 @@ class DecodeEngine:
         # device time of the decode steps (graph capture is a one-off host-side cost, reported separately)
         self.last_timing = {"steps": step, "decode_ms": ev[0].elapsed_time(ev[1]) + ev[2].elapsed_time(ev[3]),
                             "capture_ms": ev[1].elapsed_time(ev[2]), "cuda_graph": graph is not None}
+        if lpb is not None:
+            return out_ids, out_img, [lpb.take(b, 0, n_ids[b], int(logprobs)) for b in range(B)]
         return out_ids, out_img

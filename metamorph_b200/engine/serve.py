@@ -23,6 +23,10 @@ A paged server also caches prompt prefixes: `h = cache_prefix(prefix)` prefills 
 `submit(suffix, prefix=h)` shares them and prefills only the prefix tail and the suffix (attention reads the shared
 keys through the block table, `ops.attn_fwd_paged`), and `drop_prefix(h)` lets the blocks go once no request uses them.
 The request returns the bits of the whole prompt submitted without a prefix.
+A request may ask for token log-probabilities (`submit(..., logprobs=n)`): while one is in flight the step runs a graph
+that adds the logprob kernel after the state step (captured the first time it is needed, for the greedy and the sampled
+step alike); its slot's `n_top` is written on admission, -1 for every request that did not ask. The kernel only reads
+the logits and the state, so ids and embeddings keep their bits, and the reported bits do not depend on the neighbours.
 Every request's output equals what `greedy_decode` produces for it alone (tests/test_decode_gpu.py), a forced schedule
 shorter than the run included: in both, the request free-runs once its schedule ends (tests/test_serve_lifecycle_gpu.py).
 """
@@ -39,6 +43,7 @@ from ..constants import EOS_TOKEN_IDS, IMAGE_END_TOKEN_ID, IMAGE_START_TOKEN_ID
 from .decode import check_forced_tokens
 from .decode_step import decode_heads, decoder_stack_step
 from .llama import PagedPrefill, StackContext
+from .logprobs import LogprobBuffers, TokenLogprobs, cat as cat_logprobs, check_logprobs
 from .sampling import SamplingArrays, SamplingParams
 
 
@@ -62,11 +67,13 @@ class _Request:
     forced: Optional[torch.Tensor]       # [n] int32 (host) or None
     sampling: Optional[SamplingParams] = None
     prefix: Optional[PrefixHandle] = None   # positions 0 .. start-1 are this prefix's shared blocks (start = shared_len)
+    logprobs: Optional[int] = None       # alternatives reported per emitted id, None = no log-probabilities
     slot: int = -1
     sent_ids: int = 0
     sent_img: int = 0
     ids: List[torch.Tensor] = field(default_factory=list)
     img: List[torch.Tensor] = field(default_factory=list)
+    lps: List[TokenLogprobs] = field(default_factory=list)
 
 
 class KVBlockAllocator:
@@ -220,23 +227,33 @@ class ContinuousBatcher:
         self.use_cuda_graph = use_cuda_graph
         self._warm = False
         self._warm_sampled = False
+        self.lp: Optional[LogprobBuffers] = None   # allocated when the first request asks for log-probabilities
+        self.lp_graphs: Dict[bool, torch.cuda.CUDAGraph] = {}   # sampled -> step graph with the logprob kernel
+        self._warm_lp = set()
 
     # ------------------------------------------------------------------ one device step for all slots
-    def _step_body(self, sampled: bool = False):
+    def _step_body(self, sampled: bool = False, logprobs: bool = False):
         st = self.st
         x = decoder_stack_step(self.layers, self.xin, self.kc, self.vc, st["pos"] - 1, self.stack, self.table)
         tok, pred_z, prediction = decode_heads(self.m, x, st["in_image_mode"], self.logits, self.V,
                                                self.samp if sampled else None, st["total_output"])
         ops.decode_state_step_slots(st, tok, self.forced, self.max_new_slot, self.B, self.ntok, self.start_id,
                                     self.end_id, self.eos0, self.eos1, pred_z, self.img_out)
+        if logprobs:
+            self.lp.launch(self.logits, self.V, st)
         ops.decode_next_input(st["append_kind"], st["next_token"], self.inner.embed_tokens.weight.data, prediction,
                               self.xin)
 
     def _device_step(self):
         # the sampled step only while a sampled request holds a slot (finished slots are frozen: either step is fine)
         sampled = any(r is not None and r.sampling is not None for r in self.slots)
-        graph = self.sampled_graph if sampled else self.graph
-        warm = self._warm_sampled if sampled else self._warm
+        # the logprob step only while a request that asked holds a slot (the kernel skips every other row)
+        lp = any(r is not None and r.logprobs is not None for r in self.slots)
+        if lp:
+            graph, warm = self.lp_graphs.get(sampled), sampled in self._warm_lp
+        else:
+            graph = self.sampled_graph if sampled else self.graph
+            warm = self._warm_sampled if sampled else self._warm
         if graph is not None:
             graph.replay()
         elif self.use_cuda_graph and warm:
@@ -244,8 +261,10 @@ class ContinuousBatcher:
             g = torch.cuda.CUDAGraph()
             try:
                 with torch.cuda.graph(g):
-                    self._step_body(sampled)
-                if sampled:                            # (the capture itself does not execute the step)
+                    self._step_body(sampled, lp)
+                if lp:                                 # (the capture itself does not execute the step)
+                    self.lp_graphs[sampled] = g
+                elif sampled:
                     self.sampled_graph = g
                 else:
                     self.graph = g
@@ -253,10 +272,12 @@ class ContinuousBatcher:
             except Exception:  # noqa: BLE001 - capture unsupported: stay on stream launches
                 self.use_cuda_graph = False
                 torch.cuda.synchronize()
-                self._step_body(sampled)
+                self._step_body(sampled, lp)
         else:
-            self._step_body(sampled)                   # first step of each kind eager: sets kernel attributes
-            if sampled:
+            self._step_body(sampled, lp)               # first step of each kind eager: sets kernel attributes
+            if lp:
+                self._warm_lp.add(sampled)
+            elif sampled:
                 self._warm_sampled = True
             else:
                 self._warm = True
@@ -266,7 +287,7 @@ class ContinuousBatcher:
     @torch.no_grad()
     def submit(self, inputs_embeds: torch.Tensor, max_new_tokens: Optional[int] = None,
                forced_tokens: Optional[torch.Tensor] = None, sampling: Optional[SamplingParams] = None,
-               prefix: Optional[PrefixHandle] = None) -> int:
+               prefix: Optional[PrefixHandle] = None, logprobs: Optional[int] = None) -> int:
         """inputs_embeds: [P, H] or [1, P, H] prompt embeddings (text + projected image rows, as `generate` builds
         them). sampling: None or temperature 0 = greedy; otherwise the request draws its tokens with these parameters
         and seed, and its output is the same whatever other requests share the server. forced_tokens: integer ids
@@ -275,7 +296,10 @@ class ContinuousBatcher:
         ValueError here, before any device work, and so does a request whose KV blocks exceed a paged server's whole
         pool. prefix: a handle from this server's `cache_prefix`; the prompt is then the prefix followed by
         inputs_embeds (the suffix, at least one row), and the request returns exactly what that whole prompt submitted
-        without a prefix returns. Returns the request id."""
+        without a prefix returns. logprobs: None, or an int n in [0, 20]: the request also reports, for every id it
+        emits, its log-probability and the n most likely ids with theirs (`run()` yields them as 'logprobs' chunks and
+        the 'done' payload gains a TokenLogprobs); its ids and embeddings do not change. Returns the request id."""
+        check_logprobs(logprobs)
         check_forced_tokens(forced_tokens, self.inner.embed_tokens.weight.shape[0])
         if sampling is not None and not isinstance(sampling, SamplingParams):
             raise ValueError("sampling must be a SamplingParams or None")
@@ -302,12 +326,14 @@ class ContinuousBatcher:
         if prefix is not None:
             e = torch.cat([prefix.tail, e])
         f = None if forced_tokens is None else forced_tokens.reshape(-1).to(torch.int32).cpu()
+        if logprobs is not None and self.lp is None:
+            self.lp = LogprobBuffers(self.B, self.max_ids, self.dev)
         rid = self.next_rid
         self.next_rid += 1
         if prefix is not None:
             self.alloc.ref(prefix.pid, rid)
         self.queue.append(_Request(rid, e, n_new, f, sampling if sampling is not None and not sampling.greedy else None,
-                                   prefix=prefix))
+                                   prefix=prefix, logprobs=None if logprobs is None else int(logprobs)))
         return rid
 
     # ------------------------------------------------------------------ cached prefixes
@@ -414,6 +440,8 @@ class ContinuousBatcher:
         self.st["pos"][b] = P                       # the fed token sits at position P-1
         self.max_new_slot[b] = req.max_new_tokens
         self.samp.set(b, req.sampling)
+        if self.lp is not None:
+            self.lp.set(b, req.logprobs)
         req.slot, req.sent_ids, req.sent_img = b, 0, 0
         self.slots[b] = req
 
@@ -433,6 +461,11 @@ class ContinuousBatcher:
         """One host sync: new ids / visual embeddings of every running request + the requests that finished."""
         snap = torch.stack([self.st["finished"], self.st["n_ids"], self.st["n_img"]]).cpu()
         events, done = [], []
+        # the new log-probabilities of every request that asked, in one gather per buffer
+        lp_rows = [(b, req, req.sent_ids, int(snap[1, b])) for b, req in enumerate(self.slots)
+                   if req is not None and req.logprobs is not None and int(snap[1, b]) > req.sent_ids]
+        lp_chunks = self.lp.gather([(b, lo, hi, req.logprobs) for b, req, lo, hi in lp_rows]) if lp_rows else []
+        lp_of = {b: c for (b, _, _, _), c in zip(lp_rows, lp_chunks)}
         for b, req in enumerate(self.slots):
             if req is None:
                 continue
@@ -441,6 +474,9 @@ class ContinuousBatcher:
                 chunk = self.st["ids_out"][b, req.sent_ids:n_ids].clone()
                 req.ids.append(chunk)
                 events.append((req.rid, "ids", chunk))
+                if b in lp_of:
+                    req.lps.append(lp_of[b])
+                    events.append((req.rid, "logprobs", lp_of[b]))
                 req.sent_ids = n_ids
             if n_img > req.sent_img:
                 chunk = self.img_out[b, req.sent_img:n_img].clone()
@@ -454,7 +490,9 @@ class ContinuousBatcher:
     @torch.no_grad()
     def run(self, max_steps: Optional[int] = None):
         """Generator: serves the queue; yields (rid, 'ids' | 'image_embeds', tensor) as outputs appear and
-        (rid, 'done', (ids, image_embeds)) when a request completes. Returns when queue and slots are empty."""
+        (rid, 'done', (ids, image_embeds)) when a request completes. A request submitted with logprobs= also gets
+        (rid, 'logprobs', TokenLogprobs) after each 'ids' chunk, and its 'done' payload is (ids, image_embeds,
+        TokenLogprobs). Returns when queue and slots are empty."""
         steps = 0
         while self.queue or any(s is not None for s in self.slots):
             b = self._next_admission()
@@ -477,7 +515,10 @@ class ContinuousBatcher:
                     self.table[b].fill_(self.alloc.scratch)
                 ids = torch.cat(req.ids) if req.ids else torch.empty(0, dtype=torch.int32, device=self.dev)
                 img = torch.cat(req.img) if req.img else torch.empty((0, self.C), dtype=torch.bfloat16, device=self.dev)
-                yield (req.rid, "done", (ids, img))
+                if req.logprobs is not None:
+                    yield (req.rid, "done", (ids, img, cat_logprobs(req.lps, req.logprobs, self.dev)))
+                else:
+                    yield (req.rid, "done", (ids, img))
             if max_steps is not None and steps >= max_steps:
                 return
 

@@ -27,6 +27,7 @@ import torch.nn as nn
 from .. import ops
 from ..constants import EOS_TOKEN_IDS, IGNORE_INDEX, IMAGE_END_TOKEN_ID, IMAGE_START_TOKEN_ID, VISION_FEATURE_DIM
 from ..engine.decode import DecodeEngine
+from ..engine.logprobs import check_logprobs
 from ..engine.hot_path import GradProvider, HotPath
 from ..engine.llama import LlamaDims, LlamaStack, StackContext
 from ..engine.packing import deinterleave_gate_up, interleave_gate_up
@@ -427,27 +428,37 @@ class MetaMorphLlamaForCausalLM(nn.Module, MetaMorphMetaForCausalLM):
                       start_image_token_id=IMAGE_START_TOKEN_ID, end_image_token_id=IMAGE_END_TOKEN_ID,
                       eos_token_id=list(EOS_TOKEN_IDS), do_sample=None, temperature=None, top_p=None,
                       num_beams=None, max_new_tokens=1024, use_cache=None, output_image=False,
-                      prompt_lens=None, forced_tokens=None, sampling=None):
+                      prompt_lens=None, forced_tokens=None, sampling=None, logprobs=None):
         """metamorph_llama.py:502-597 with a KV cache; accepts a batch (<= 8) of right-padded prompts.
         sampling: None (greedy, as the reference), a SamplingParams (sequence b draws with seed + b) or one per
         sequence (metamorph_b200.engine.sampling). The seeded draw replaces the argmax of metamorph_llama.py:542 and
         nothing else. `do_sample`, `temperature` and `top_p` are accepted and ignored, as the reference's
-        greedy_decode ignores them: sampling is asked for with `sampling=` only."""
-        ids, imgs = self._decode.generate(inputs_embeds, prompt_lens=prompt_lens, max_new_tokens=max_new_tokens,
-                                          start_image_token_id=start_image_token_id,
-                                          end_image_token_id=end_image_token_id, eos_token_id=eos_token_id,
-                                          forced_tokens=forced_tokens, sampling=sampling)
+        greedy_decode ignores them: sampling is asked for with `sampling=` only.
+        logprobs: None, or an int n in [0, 20]: the list of TokenLogprobs per sequence (engine/logprobs.py) is appended
+        as the last return element; without it the return convention is the reference's."""
+        res = self._decode.generate(inputs_embeds, prompt_lens=prompt_lens, max_new_tokens=max_new_tokens,
+                                    start_image_token_id=start_image_token_id,
+                                    end_image_token_id=end_image_token_id, eos_token_id=eos_token_id,
+                                    forced_tokens=forced_tokens, sampling=sampling, logprobs=logprobs)
+        ids, imgs = res[0], res[1]
         B = inputs_embeds.shape[0]
         if B == 1:  # reference return convention: [ids] and a [n, 1152] tensor
             img = imgs[0] if imgs[0].shape[0] > 0 else torch.tensor([], dtype=torch.float32, device=inputs_embeds.device)
-            return (ids[:1], img) if output_image else ids[:1]
-        return (ids, imgs) if output_image else ids
+            out = (ids[:1], img) if output_image else (ids[:1],)
+            lps = res[2][:1] if logprobs is not None else None
+        else:
+            out = (ids, imgs) if output_image else (ids,)
+            lps = res[2] if logprobs is not None else None
+        if lps is not None:
+            return out + (lps,)
+        return out if output_image else out[0]
 
     @torch.no_grad()
     def generate(self, inputs=None, images=None, image_sizes=None, output_image=False,
                  use_customize_greedy=True, image_embeds=None, **kwargs):
         """metamorph_llama.py:666-717. Pass `sampling=SamplingParams(...)` (forwarded to greedy_decode) to sample;
         `do_sample` / `temperature` / `top_p` are dropped on this custom-greedy path, as in the reference."""
+        check_logprobs(kwargs.get("logprobs"))
         position_ids = kwargs.pop("position_ids", None)
         attention_mask = kwargs.pop("attention_mask", None)
         prompt_lens = None

@@ -288,6 +288,29 @@ def sample_rows(logits_f32, V, temperature, top_k, top_p, seed, counter, out=Non
     return out
 
 
+LOGPROB_TOP_MAX = 20
+
+
+def decode_logprobs(logits_f32, V, append_kind, token, n_ids, n_top, lp_out, top_ids, top_lp):
+    """Log-probabilities of the tokens a decode step appended (csrc/sampling.cu, DESIGN.md's log-probability
+    contract). Row r with append_kind[r] == 0 and n_top[r] >= 0 writes lp_out[r, n_ids[r] - 1] = the raw
+    log-softmax of token[r] and the first min(n_top[r], 20) entries of top_ids / top_lp [r, n_ids[r] - 1, :]; a slot
+    past lp_out's max_ids columns and every other row are left untouched. Per-row int32 device arrays; lp_out fp32
+    [R, max_ids], top_ids int32 / top_lp fp32 [R, max_ids, 20], contiguous."""
+    require_cuda(logits_f32, append_kind, token, n_ids, n_top, lp_out, top_ids, top_lp)
+    R = logits_f32.shape[0]
+    assert logits_f32.dtype == torch.float32 and logits_f32.stride(1) == 1
+    for t in (append_kind, token, n_ids, n_top):
+        assert t.dtype == torch.int32 and t.is_contiguous() and t.numel() >= R, "decode_logprobs: bad per-row array"
+    max_ids = lp_out.shape[1]
+    assert lp_out.dtype == torch.float32 and lp_out.is_contiguous() and lp_out.shape[0] >= R
+    for t, dt in ((top_ids, torch.int32), (top_lp, torch.float32)):
+        assert t.dtype == dt and t.is_contiguous() and tuple(t.shape[1:]) == (max_ids, LOGPROB_TOP_MAX) \
+            and t.shape[0] >= R, "decode_logprobs: bad top-n buffer"
+    call("mm_decode_logprobs", ptr(logits_f32), ll(logits_f32.stride(0)), ll(R), c_int(V), ptr(append_kind),
+         ptr(token), ptr(n_ids), ptr(n_top), c_int(max_ids), ptr(lp_out), ptr(top_ids), ptr(top_lp), stream_ptr())
+
+
 # ------------------------------------------------------------------------------------------------
 # optimizer
 # ------------------------------------------------------------------------------------------------
