@@ -138,13 +138,9 @@ int mm_adamw_step_bcast(void* multicast_p16, const void* const* peers, int n_pee
 int mm_clip_coef(const float* sumsq, float* out2, float max_norm, cudaStream_t s);
 
 /* Attention: LLaMA causal GQA (modeling_llama.py:199-220) forward/backward, SigLIP MHA forward
- * (modeling_siglip.py:229-249). q/k/v/o are [B*T, heads*head_dim] views with independent pitches. */
-int mm_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, const int* seqlens,
-                long long ldq, long long ldk, long long ldv, long long ldo, int B, int T, int Hq, int Hkv,
-                int head_dim, int causal, float scale, cudaStream_t s);
-long long mm_attn_bwd_workspace_bytes(int B, int T, int Hq);
-/* wgmma / TMA flash attention for head_dim 128 (csrc/attention_tc.cu forward, csrc/attention_bwd_tc.cu backward:
- * a query-stationary dQ kernel + a key-stationary dK/dV kernel, no atomics -> bit-reproducible); same contracts as above.
+ * (modeling_siglip.py:229-249). q/k/v/o are [B*T, heads*head_dim] views with independent pitches.
+ * wgmma / TMA flash attention for head_dim 128 (csrc/attention_tc.cu forward, csrc/attention_bwd_tc.cu backward:
+ * a query-stationary dQ kernel + a key-stationary dK/dV kernel, no atomics -> bit-reproducible).
  * Rows >= seqlens[b] are outside the sequence: zero dQ/dK/dV, their dO is ignored. Backward workspace: lse*log2e and
  * delta, mm_attn_bwd_tc_workspace_bytes. */
 long long mm_attn_bwd_tc_workspace_bytes(int B, int T, int Hq);
@@ -170,11 +166,6 @@ int mm_attn_bwd_tc_varlen(const void* q, const void* k, const void* v, const voi
                           long long total_rows, long long ldq, long long ldk, long long ldv, long long ldo,
                           long long lddo, long long lddq, long long lddk, long long lddv, int Hq, int Hkv,
                           int head_dim, float scale, void* workspace, long long workspace_bytes, cudaStream_t s);
-int mm_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
-                void* dq, void* dk, void* dv, const int* seqlens, long long ldq, long long ldk, long long ldv,
-                long long ldo, long long lddo, long long lddq, long long lddk, long long lddv, int B, int T,
-                int Hq, int Hkv, int head_dim, float scale, void* workspace, long long workspace_bytes,
-                cudaStream_t s);
 
 /* On-GPU SigLIP image pre-processing (SURVEY.md section 8f, row N1), bit-exact with the reference's CPU chain:
  * expand2square + processor.preprocess (metamorph/train/train.py:1189-1209) with the SigLIP processor of

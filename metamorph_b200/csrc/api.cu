@@ -1,6 +1,5 @@
 // metamorph_b200 — C-ABI plumbing shared by all kernels: thread-local error text, device queries.
 #include "common.cuh"
-#include <stdlib.h>
 #include <stdarg.h>
 #include <map>
 #include <mutex>
@@ -16,23 +15,6 @@ void mm_set_error(const char* fmt, ...) {
 }
 
 MM_API const char* mm_last_error() { return g_err; }
-
-int mm_pdl_enabled() {
-  static const int on = [] {
-    const char* e = getenv("MM_PDL");
-    return (e && e[0] == '0') ? 0 : 1;
-  }();
-  return on;
-}
-
-int mm_pdl_mode() {
-  static const int mode = [] {
-    if (!mm_pdl_enabled()) return 0;
-    const char* e = getenv("MM_PDL_MODE");
-    return e ? atoi(e) : 3;
-  }();
-  return mode;
-}
 
 int mm_num_sms() {
   static int sms = 0;

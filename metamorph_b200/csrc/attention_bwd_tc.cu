@@ -447,7 +447,8 @@ int launch_bwd_tc(const void* q, const void* k, const void* v, const void* o, co
 
 }  // namespace
 
-// wgmma flash-attention backward; same argument meaning as mm_attn_bwd (workspace from mm_attn_bwd_tc_workspace_bytes).
+// wgmma flash-attention backward (workspace from mm_attn_bwd_tc_workspace_bytes). See include/metamorph_b200.h for the
+// contract.
 MM_API int mm_attn_bwd_tc(const void* q, const void* k, const void* v, const void* o, const void* dout,
                           const float* lse, void* dq, void* dk, void* dv, const int* seqlens, long long ldq,
                           long long ldk, long long ldv, long long ldo, long long lddo, long long lddq,

@@ -355,7 +355,7 @@ int paged_block_shift(int block_size) {
 
 }  // namespace
 
-// wgmma flash-attention forward, head_dim 128. Same argument meaning as mm_attn_fwd.
+// wgmma flash-attention forward, head_dim 128. See include/metamorph_b200.h for the contract.
 MM_API int mm_attn_fwd_tc(const void* q, const void* k, const void* v, void* o, float* lse,
                           const int* seqlens, long long ldq, long long ldk, long long ldv, long long ldo,
                           int B, int T, int Hq, int Hkv, int head_dim, int causal, float scale,

@@ -1,5 +1,5 @@
 // metamorph_b200 — shared device/host helpers for the sm_90a kernels.
-// Hand-written for Hopper (H100): mbarrier, TMA, cp.async / ldmatrix / mma.sync PTX wrappers,
+// Hand-written for Hopper (H100): mbarrier, TMA and mma.sync PTX wrappers,
 // warp-shuffle reductions, 128-bit global access helpers and the C-ABI error plumbing (wgmma lives in wgmma.cuh).
 #pragma once
 #include <cuda_runtime.h>
@@ -52,12 +52,6 @@ int mm_num_sms();
 // share it. nullptr (with the error text set) when the allocation fails.
 void* mm_stream_scratch(int tag, size_t bytes, cudaStream_t stream);
 enum { MM_SCRATCH_LOSS = 0, MM_SCRATCH_RMSNORM_DW = 1, MM_SCRATCH_SUMSQ = 2 };
-// programmatic dependent launch (PDL) for the decode chain: 1 unless MM_PDL=0 (api.cu)
-int mm_pdl_enabled();
-// MM_PDL_MODE bitmask (default 3): 1 = weight-streaming GEMMs launched with the PDL attribute, 2 = the small decode kernels
-// too, 8 = trigger dependents after the main loop instead of at kernel entry. The early trigger lets the next kernel's
-// producer fill its ring with weights while this one drains.
-int mm_pdl_mode();
 
 // ----------------------------------------------------------------------------------------------
 // Device helpers
@@ -74,7 +68,7 @@ __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefe
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 template <typename... KArgs, typename... Args>
-static inline cudaError_t launch_pdl(int allow, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
+static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
                                      cudaStream_t stream, Args... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
@@ -83,7 +77,7 @@ static inline cudaError_t launch_pdl(int allow, void (*kernel)(KArgs...), dim3 g
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = allow ? 1 : 0;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
@@ -236,32 +230,7 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const void* tmap,
       : "memory");
 }
 
-// ---------------------------------------------------------------- cp.async / ldmatrix / mma.sync
-__device__ __forceinline__ void cp_async16(uint32_t smem_dst, const void* gsrc, bool pred) {
-  const int sz = pred ? 16 : 0;  // src-size 0 => zero fill
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_dst), "l"(gsrc),
-               "r"(sz)
-               : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() {
-  asm volatile("cp.async.commit_group;" ::: "memory");
-}
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2,
-                                        uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
-               : "r"(addr));
-}
-__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t& r0, uint32_t& r1,
-                                          uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
-               : "r"(addr));
-}
+// ---------------------------------------------------------------- mma.sync
 // D(16x8,f32) += A(16x16,bf16,row) * B(16x8,bf16,col)
 __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0,
                                                uint32_t b1) {

@@ -39,8 +39,7 @@ template <int ROWS, int NST = SK2_STAGES, int NB = 1>
 __global__ void __launch_bounds__(SK2_THREADS)
 skinny_gemm_tma_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
                        void* __restrict__ y, long long ldy, const bf16* __restrict__ bias,
-                       const bf16* __restrict__ resid, long long ldr, int m, int N, int K, int epi, int out_f32,
-                       int pdl) {
+                       const bf16* __restrict__ resid, long long ldr, int m, int N, int K, int epi, int out_f32) {
   constexpr int G = ROWS >= 16 ? ROWS / 16 : 1;
   constexpr bool HALF = ROWS == 8;             // 8-row slab: rows 8..15 of the MMA operand are zero
   constexpr int MB = 8 * NB;                   // batch rows served: NB n8 tiles of the MMA's B operand
@@ -66,7 +65,7 @@ skinny_gemm_tma_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
     }
     fence_barrier_init();
   }
-  if (!(pdl & 8)) griddep_launch();
+  griddep_launch();
   __syncthreads();
   if (warp == 0) {
     if (lane == 0) {
@@ -160,7 +159,6 @@ skinny_gemm_tma_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
   }
   griddep_wait();
   __syncthreads();
-  if (pdl & 8) griddep_launch();
   if (epi == SK_SWIGLU) {
     if (ROWS >= 32) {
       // rows of the slab: [16 gate | 16 up] per group of 32 (engine/packing.py interleave_gate_up)
@@ -546,7 +544,7 @@ namespace {
 
 template <int ROWS, int NST, int NB>
 int launch_skinny_tma(const CUtensorMap& tw, const CUtensorMap& tx, void* y, long long ldy, const void* bias,
-                      const void* resid, long long ldr, int m, int N, int K, int epilogue, int out_f32, int pm,
+                      const void* resid, long long ldr, int m, int N, int K, int epilogue, int out_f32,
                       cudaStream_t stream) {
   constexpr int smem = NST * (4 * ROWS * 128 + 4 * 8 * NB * 128) + ((2 * NST * 8 + 127) & ~127) + 4 * ROWS * 8 * NB * 4 + 1024;
   static_assert(smem <= 227 * 1024, "skinny GEMM ring does not fit in shared memory");
@@ -556,9 +554,8 @@ int launch_skinny_tma(const CUtensorMap& tw, const CUtensorMap& tx, void* y, lon
     err = cudaFuncSetAttribute(skinny_gemm_tma_kernel<ROWS, NST, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   });
   MM_CHECK_CUDA(err);
-  MM_CHECK_CUDA(launch_pdl(pm & 1, skinny_gemm_tma_kernel<ROWS, NST, NB>, dim3((N + ROWS - 1) / ROWS), dim3(SK2_THREADS),
-                           smem, stream, tw, tx, y, ldy, (const bf16*)bias, (const bf16*)resid, ldr, m, N, K, epilogue,
-                           out_f32, pm));
+  MM_CHECK_CUDA(launch_pdl(skinny_gemm_tma_kernel<ROWS, NST, NB>, dim3((N + ROWS - 1) / ROWS), dim3(SK2_THREADS), smem,
+                           stream, tw, tx, y, ldy, (const bf16*)bias, (const bf16*)resid, ldr, m, N, K, epilogue, out_f32));
   MM_CHECK_LAUNCH();
   return MM_OK;
 }
@@ -574,7 +571,6 @@ MM_API int mm_skinny_gemm(const void* x, const void* W, void* y, const void* bia
   MM_CHECK_ARG(epilogue >= SK_STORE && epilogue <= SK_SWIGLU, "mm_skinny_gemm: bad epilogue");
   MM_CHECK_ARG((epilogue != SK_BIAS && epilogue != SK_BIAS_GELU) || bias, "mm_skinny_gemm: bias missing");
   MM_CHECK_ARG(epilogue != SK_RESID || resid, "mm_skinny_gemm: residual missing");
-  const int pm = mm_pdl_mode();
   // The batch is the n dimension of the MMA: 1, 2 or 4 n8 tiles (8 / 16 / 32 sequences) share every weight fragment.
   const int nb = m <= 8 ? 1 : (m <= 16 ? 2 : 4);
   // 32-row slabs where the epilogue needs them (SwiGLU: 16 gate + 16 up rows of the same channels), for very large N
@@ -617,7 +613,7 @@ MM_API int mm_skinny_gemm(const void* x, const void* W, void* y, const void* bia
   }
   // Ring depths: as deep as keeps two CTAs per SM (profiles/r02_decode_skinny_ring_sweep.txt: deeper rings bought nothing);
   // 32 sequences: 32 KB (32-row slabs) or 48 KB (64-row slabs) stages, one CTA per SM.
-#define MM_SK(R, S, B) return launch_skinny_tma<R, S, B>(tw, tx, y, ldy, bias, resid, ldr, m, N, K, epilogue, out_f32, pm, stream)
+#define MM_SK(R, S, B) return launch_skinny_tma<R, S, B>(tw, tx, y, ldy, bias, resid, ldr, m, N, K, epilogue, out_f32, stream)
   if (rows64) MM_SK(64, 4, 4);
   if (nb == 4) MM_SK(32, 5, 4);
   if (nb == 2) {
@@ -656,7 +652,7 @@ int decode_attn_launch(const char* name, const void* qkv, long long ldqkv, void*
     if (smem > 48 * 1024)                                                                                    \
       MM_CHECK_CUDA(cudaFuncSetAttribute(decode_attn_kernel<GG, PAGED>,                                      \
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));           \
-    MM_CHECK_CUDA(launch_pdl(mm_pdl_mode() & 2, decode_attn_kernel<GG, PAGED>, grid, dim3(DA_THREADS), smem, stream, \
+    MM_CHECK_CUDA(launch_pdl(decode_attn_kernel<GG, PAGED>, grid, dim3(DA_THREADS), smem, stream,            \
                              (const bf16*)qkv, ldqkv, (bf16*)kcache, (bf16*)vcache, pos, cos_t, sin_t,       \
                              (float*)workspace, Hq, Hkv, Tmax, splits, scale, table, max_blocks, bs_shift));  \
   } while (0)
@@ -666,7 +662,7 @@ int decode_attn_launch(const char* name, const void* qkv, long long ldqkv, void*
   else MM_DA_LAUNCH(8);
 #undef MM_DA_LAUNCH
   MM_CHECK_LAUNCH();
-  MM_CHECK_CUDA(launch_pdl(mm_pdl_mode() & 2, decode_attn_combine_kernel, dim3(Hkv, B), dim3(128), 0, stream, (const float*)workspace,
+  MM_CHECK_CUDA(launch_pdl(decode_attn_combine_kernel, dim3(Hkv, B), dim3(128), 0, stream, (const float*)workspace,
                            (bf16*)out, ldo, Hkv, G, splits));
   MM_CHECK_LAUNCH();
   return MM_OK;

@@ -42,8 +42,7 @@ static_assert(kMB * kPLd * 4 <= kStages * kStageBytes, "the partial tile reuses 
 __global__ void __launch_bounds__(kThreads, 2)
 skinny_gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
                         void* __restrict__ y, long long ldy, const bf16* __restrict__ bias,
-                        const bf16* __restrict__ resid, long long ldr, int m, int N, int K, int epi, int out_f32,
-                        int pdl) {
+                        const bf16* __restrict__ resid, long long ldr, int m, int N, int K, int epi, int out_f32) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
@@ -64,7 +63,7 @@ skinny_gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid
     }
     fence_barrier_init();
   }
-  if (!(pdl & 8)) griddep_launch();
+  griddep_launch();
   __syncthreads();
   float d[64];
   if (warp == 8) {
@@ -106,7 +105,6 @@ skinny_gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid
       if (lane == 0) mbar_arrive(bar + 8 * (kStages + s));
     }
   }
-  if (pdl & 8) griddep_launch();
   __syncthreads();                               // every stage has been consumed: the ring holds the partial tile now
   float* part = reinterpret_cast<float*>(base_ptr);   // [kMB batch rows][kPLd] fp32, weight row fastest
   if (warp < 8) {
@@ -242,7 +240,6 @@ MM_API int mm_skinny_gemm_wide(const void* x, const void* W, void* y, const void
   });
   MM_CHECK_CUDA(attr_err);
   const int S = wide_splits(N, K);
-  const int pm = mm_pdl_mode();
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)(((N + kRows - 1) / kRows) * S));
   cfg.blockDim = dim3(kThreads);
@@ -254,11 +251,11 @@ MM_API int mm_skinny_gemm_wide(const void* x, const void* W, void* y, const void
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = (pm & 1) ? 1 : 0;
+  attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 2;
   MM_CHECK_CUDA(cudaLaunchKernelEx(&cfg, skinny_gemm_wide_kernel, tw, tx, y, ldy, (const bf16*)bias,
-                                   (const bf16*)resid, ldr, m, N, K, epilogue, out_f32, pm));
+                                   (const bf16*)resid, ldr, m, N, K, epilogue, out_f32));
   MM_CHECK_LAUNCH();
   return MM_OK;
 }

@@ -18,7 +18,6 @@
 //                             thread -> epilogue_chunk -> global)
 #include "wgmma.cuh"
 #include <mutex>
-#include <stdlib.h>
 
 namespace {
 
@@ -400,11 +399,6 @@ int make_tmap(CUtensorMap* tm, const void* base, long long inner, long long oute
   return MM_OK;
 }
 
-int env_group_m() {   // MM_GEMM_GM: rasterisation group size override (experiments; read once per process)
-  static const int v = [] { const char* e = getenv("MM_GEMM_GM"); return e ? atoi(e) : 0; }();
-  return v;
-}
-
 template <int BN, bool A_MN, bool B_MN>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, const EpiParams& ep,
            cudaStream_t stream) {
@@ -425,7 +419,6 @@ int launch(const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, co
   long long gm = (16ll << 20) / ((long long)BM * K * 2);
   if (gm < 11) gm = 11;
   if (gm > 64) gm = 64;
-  if (env_group_m() > 0) gm = env_group_m();
   kern<<<grid, kThreads, Cfg<BN>::kSmemBytes, stream>>>(ta, tb, M, N, K, (int)gm, ep);
   MM_CHECK_LAUNCH();
   return MM_OK;

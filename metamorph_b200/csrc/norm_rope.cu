@@ -311,8 +311,8 @@ MM_API int mm_rmsnorm_fwd(const void* x, const void* w, void* y, long long M, lo
   const int cap = mm_num_sms() * (vpt <= 2 ? 8 : 2);     // resident blocks per SM x 2 (tail balance)
   const dim3 grid(M < cap ? (int)M : cap);
 #define MM_RMS_FWD(V)                                                                                                \
-  MM_CHECK_CUDA(launch_pdl(mm_pdl_mode() & 2, rmsnorm_fwd_kernel<V>, grid, dim3(kNormThreads), 0, stream, (const bf16*)x, \
-                           (const bf16*)w, (bf16*)y, (int)M, (int)H, eps))
+  MM_CHECK_CUDA(launch_pdl(rmsnorm_fwd_kernel<V>, grid, dim3(kNormThreads), 0, stream, (const bf16*)x, (const bf16*)w,    \
+                           (bf16*)y, (int)M, (int)H, eps))
   if (vpt <= 1) MM_RMS_FWD(1);
   else if (vpt == 2) MM_RMS_FWD(2);
   else MM_RMS_FWD(4);

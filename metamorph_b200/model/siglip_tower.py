@@ -182,7 +182,7 @@ class SiglipVisionTransformerParams(nn.Module):
             h = ops.layernorm(x, l.layer_norm1.weight.data, l.layer_norm1.bias.data, c.layer_norm_eps)
             qkv = ops.gemm(h, pl["wqkv"], bias=pl["bqkv"], epilogue=ops.EPI_BIAS)
             attn, _ = ops.attn_fwd(qkv[:, :Wp], qkv[:, Wp:2 * Wp], qkv[:, 2 * Wp:], n, P, heads, heads, pk["head_slot"],
-                                   False, scale, need_lse=False, tc=True)
+                                   False, scale, need_lse=False)
             x = ops.gemm(attn, pl["wo"], bias=l.self_attn.out_proj.bias.data, resid=x, epilogue=ops.EPI_BIAS_RESID)
             h = ops.layernorm(x, l.layer_norm2.weight.data, l.layer_norm2.bias.data, c.layer_norm_eps)
             h = ops.gemm(h, l.mlp.fc1.weight.data, bias=l.mlp.fc1.bias.data, epilogue=ops.EPI_BIAS_GELU_TANH)

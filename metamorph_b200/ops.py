@@ -12,8 +12,6 @@ from ._lib import c_float, c_int, c_void_p, call, ll, ptr, require_cuda, stream_
 EPI_STORE, EPI_BIAS, EPI_BIAS_GELU_ERF, EPI_BIAS_GELU_TANH, EPI_RESID, EPI_BIAS_RESID, EPI_SWIGLU, EPI_SWIGLU_BWD = range(8)
 
 
-ATTN_BWD_TC = True  # wgmma backward (csrc/attention_bwd_tc.cu); the mma.sync kernel stays selectable with tc=False
-
 # bench.py instrumentation: when a list, every GEMM launch appends (start_event, end_event, flops)
 GEMM_PROFILE = None
 
@@ -356,37 +354,34 @@ def clip_coef(sumsq, max_norm):
 # ------------------------------------------------------------------------------------------------
 # attention
 # ------------------------------------------------------------------------------------------------
-def attn_fwd(q, k, v, B, T, Hq, Hkv, head_dim, causal, scale, seqlens=None, out=None, need_lse=True,
-             tc=None):
+def attn_fwd(q, k, v, B, T, Hq, Hkv, head_dim, causal, scale, seqlens=None, out=None, need_lse=True):
     """q/k/v: 2-D row-major views [B*T, *] (may be column slices of one fused QKV buffer)."""
     require_cuda(q, k, v, seqlens)
     assert q.stride(1) == 1 and k.stride(1) == 1 and v.stride(1) == 1
     if out is None:
         out = torch.empty((B * T, Hq * head_dim), dtype=torch.bfloat16, device=q.device)
     lse = torch.empty((B, Hq, T), dtype=torch.float32, device=q.device) if need_lse else None
-    # One kernel on the product path: wgmma, 128-wide head slots (narrower heads are zero-padded into such slots by their
-    # caller, as SiglipVisionTower does). tc=False selects the mma.sync comparison kernels (tests / microbenchmarks only).
-    use_tc = True if tc is None else tc
-    if use_tc and head_dim != 128:
+    # The wgmma kernel takes 128-wide head slots: narrower heads are zero-padded into such slots by their caller, as
+    # SiglipVisionTower does.
+    if head_dim != 128:
         raise ValueError(f"attn_fwd: the wgmma attention takes head_dim 128 (got {head_dim}); pad the heads into 128-wide "
-                         "slots or pass tc=False for the mma.sync comparison kernel")
-    call("mm_attn_fwd_tc" if use_tc else "mm_attn_fwd", ptr(q), ptr(k), ptr(v), ptr(out), ptr(lse), ptr(seqlens), ll(q.stride(0)),
+                         "slots")
+    call("mm_attn_fwd_tc", ptr(q), ptr(k), ptr(v), ptr(out), ptr(lse), ptr(seqlens), ll(q.stride(0)),
          ll(k.stride(0)), ll(v.stride(0)), ll(out.stride(0)), c_int(B), c_int(T), c_int(Hq),
          c_int(Hkv), c_int(head_dim), c_int(int(causal)), c_float(scale), stream_ptr())
     return out, lse
 
 
 def attn_bwd(q, k, v, o, dout, lse, dq, dk, dv, B, T, Hq, Hkv, head_dim, scale, seqlens=None,
-             workspace=None, tc=None):
+             workspace=None):
     require_cuda(q, k, v, o, dout, lse, dq, dk, dv)
     from ._lib import lib
-    use_tc = ATTN_BWD_TC if tc is None else tc   # tc=False: the mma.sync kernel, kept as a test-only comparison
-    fn = lib().mm_attn_bwd_tc_workspace_bytes if use_tc else lib().mm_attn_bwd_workspace_bytes
+    fn = lib().mm_attn_bwd_tc_workspace_bytes
     fn.restype = ctypes_ll
     need = fn(c_int(B), c_int(T), c_int(Hq))
     if workspace is None or workspace.numel() < need:
         workspace = torch.empty(need, dtype=torch.uint8, device=q.device)
-    call("mm_attn_bwd_tc" if use_tc else "mm_attn_bwd", ptr(q), ptr(k), ptr(v), ptr(o), ptr(dout), ptr(lse), ptr(dq), ptr(dk), ptr(dv),
+    call("mm_attn_bwd_tc", ptr(q), ptr(k), ptr(v), ptr(o), ptr(dout), ptr(lse), ptr(dq), ptr(dk), ptr(dv),
          ptr(seqlens), ll(q.stride(0)), ll(k.stride(0)), ll(v.stride(0)), ll(o.stride(0)),
          ll(dout.stride(0)), ll(dq.stride(0)), ll(dk.stride(0)), ll(dv.stride(0)), c_int(B), c_int(T),
          c_int(Hq), c_int(Hkv), c_int(head_dim), c_float(scale), ptr(workspace), ll(workspace.numel()),

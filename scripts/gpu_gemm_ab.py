@@ -1,6 +1,4 @@
-"""Time the step's dominant GEMM shapes (CUDA events, L2-cold: operands > 126 MB) under the current MM_GEMM_* env:
-    MM_GEMM_DYNAMIC=0/1 (cluster-launch-control tile stealing), MM_GEMM_L2HINT=0/1 (TMA eviction hints)."""
-import os
+"""Time the step's dominant GEMM shapes (CUDA events, L2-cold: operands > 126 MB)."""
 import sys
 
 import torch
@@ -15,7 +13,6 @@ shapes = [("fwd gate/up  [M,4096]x[28672,4096]^T", (M, 28672, 4096), False, Fals
           ("dgrad gate/up [M,28672]x[28672,4096]", (M, 4096, 28672), False, True),
           ("wgrad gate/up [M,28672]^T x [M,4096]", (28672, 4096, M), True, True),
           ("fwd qkv      [M,4096]x[6144,4096]^T", (M, 6144, 4096), False, False)]
-tag = f"dynamic={os.environ.get('MM_GEMM_DYNAMIC', '1')} l2hint={os.environ.get('MM_GEMM_L2HINT', '0')}"
 for name, (m, n, k), a_mn, b_mn in shapes:
     a = (torch.randn((k, m) if a_mn else (m, k), device="cuda") * 0.1).bfloat16()
     b = (torch.randn((k, n) if b_mn else (n, k), device="cuda") * 0.1).bfloat16()
@@ -33,5 +30,5 @@ for name, (m, n, k), a_mn, b_mn in shapes:
     ms = e0.elapsed_time(e1) / it
     ref = (a.float().t() if a_mn else a.float())[:256] @ (b.float() if b_mn else b.float().t())
     err = (out[:256].float() - ref).abs().max().item() / (ref.abs().max().item() + 1e-9)
-    print(f"[{tag}] {name}: {ms:.3f} ms  {2.0 * m * n * k / ms / 1e9:.0f} TFLOP/s  rel err {err:.2e}", flush=True)
+    print(f"{name}: {ms:.3f} ms  {2.0 * m * n * k / ms / 1e9:.0f} TFLOP/s  rel err {err:.2e}", flush=True)
     del a, b, out

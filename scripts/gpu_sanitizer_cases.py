@@ -28,6 +28,17 @@ def case(name):
     return not only or name in only
 
 
+def attn_ref(q, k, v, scale, seqlens):
+    # causal GQA attention in fp32; q [B,T,Hq,d], k/v [B,T,Hkv,d]; keys >= seqlens[b] are masked
+    B, T, Hq, d = q.shape
+    k = k.repeat_interleave(Hq // k.shape[2], dim=2)
+    v = v.repeat_interleave(Hq // v.shape[2], dim=2)
+    s = torch.einsum("bqhd,bkhd->bhqk", q, k) * scale
+    mask = torch.tril(torch.ones(T, T, dtype=torch.bool, device=q.device))[None, None]
+    mask = mask & (torch.arange(T, device=q.device)[None, None, None, :] < seqlens.view(B, 1, 1, 1))
+    return torch.einsum("bhqk,bkhd->bqhd", s.masked_fill(~mask, float("-inf")).softmax(-1), v)
+
+
 if case("gemm"):
     for force, (M, N, K) in ((128, (304, 200, 136)), (256, (264, 520, 200)), (512, (512, 512, 256)), (512, (304, 264, 72))):
         a = torch.randn(M, K, device=dev).bfloat16()
@@ -45,18 +56,20 @@ if case("attn"):
         q, k, v = qkv[:, :Hq * d], qkv[:, Hq * d:(Hq + Hkv) * d], qkv[:, (Hq + Hkv) * d:]
         sl = torch.tensor([T, T - 33][:B], device=dev, dtype=torch.int32)
         out, lse = ops.attn_fwd(q, k, v, B, T, Hq, Hkv, d, True, 1 / math.sqrt(d), seqlens=sl)
-        out2, _ = ops.attn_fwd(q, k, v, B, T, Hq, Hkv, d, True, 1 / math.sqrt(d), seqlens=sl, tc=False)
-        close(out.view(B, T, -1)[0], out2.view(B, T, -1)[0], 2e-2, f"attn fwd tc vs mma.sync T={T}")
         dout = torch.randn(B * T, Hq * d, device=dev).bfloat16()
         for b in range(B):
             dout.view(B, T, -1)[b, int(sl[b]):] = 0
-        g1, g2 = torch.zeros_like(qkv), torch.zeros_like(qkv)
-        for g, tc in ((g1, True), (g2, False)):
-            ops.attn_bwd(q, k, v, out, dout, lse, g[:, :Hq * d], g[:, Hq * d:(Hq + Hkv) * d], g[:, (Hq + Hkv) * d:], B, T, Hq,
-                         Hkv, d, 1 / math.sqrt(d), seqlens=sl, tc=tc)
+        g = torch.zeros_like(qkv)
+        ops.attn_bwd(q, k, v, out, dout, lse, g[:, :Hq * d], g[:, Hq * d:(Hq + Hkv) * d], g[:, (Hq + Hkv) * d:], B, T, Hq,
+                     Hkv, d, 1 / math.sqrt(d), seqlens=sl)
+        qf, kf, vf = (t.float().view(B, T, -1, d).clone().requires_grad_(True) for t in (q, k, v))
+        ref = attn_ref(qf, kf, vf, 1 / math.sqrt(d), sl)
+        ref.backward(dout.float().view(B, T, Hq, d))
+        gref = torch.cat([t.grad.reshape(B * T, -1) for t in (qf, kf, vf)], 1)
         for b in range(B):
             L = int(sl[b])
-            close(g1.view(B, T, -1)[b, :L], g2.view(B, T, -1)[b, :L], 4e-2, f"attn bwd tc vs mma.sync T={T} b={b}")
+            close(out.view(B, T, -1)[b, :L], ref.detach().reshape(B, T, -1)[b, :L], 2e-2, f"attn fwd T={T} b={b}")
+            close(g.view(B, T, -1)[b, :L], gref.view(B, T, -1)[b, :L], 4e-2, f"attn bwd T={T} b={b}")
     segs = [(0, 150), (150, 40), (200, 130)]
     tab = ops.SegmentTables(segs, dev)
     qkv = (torch.randn(330, 4 * 128, device=dev) * 0.5).bfloat16()

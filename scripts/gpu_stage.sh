@@ -15,11 +15,7 @@ run() {  # run <seconds> <label> <cmd...>
 }
 P="python -m pytest -q -m gpu -rs"
 run 200 "attention kernels" $P tests/test_kernels_gpu.py -x -k "attention" || { echo "ABORT: attention kernels" >> "$log"; tail -30 "$log"; exit 1; }
-if ! run 240 "gemm kernels (dynamic tile schedule)" $P tests/test_kernels_gpu.py -k "gemm"; then
-  echo "!!!!! falling back to the static tile schedule (MM_GEMM_DYNAMIC=0)" >> "$log"
-  export MM_GEMM_DYNAMIC=0
-  run 240 "gemm kernels (static)" $P tests/test_kernels_gpu.py -k "gemm" || { echo "ABORT: gemm" >> "$log"; tail -30 "$log"; exit 1; }
-fi
+run 240 "gemm kernels" $P tests/test_kernels_gpu.py -k "gemm" || { echo "ABORT: gemm" >> "$log"; tail -30 "$log"; exit 1; }
 run 300 "other kernels" $P tests/test_kernels_gpu.py -k "not gemm and not attention"
 run 420 "model" $P tests/test_model_gpu.py
 run 600 "realwidth" $P tests/test_realwidth_gpu.py -s

@@ -299,13 +299,9 @@ def _attn_ref(q, k, v, causal, scale, seqlens=None):
     return torch.einsum("bhqk,bkhd->bqhd", p, v)
 
 
-@pytest.mark.parametrize("tc", [False, True])
 @pytest.mark.parametrize("B,T,Hq,Hkv,d,causal", [(2, 300, 8, 2, 128, True), (1, 1024, 4, 4, 128, True),
-                                                 (2, 729, 4, 4, 72, False), (1, 200, 2, 2, 64, False),
                                                  (2, 640, 4, 2, 128, False)])
-def test_attention_fwd(cuda_device, B, T, Hq, Hkv, d, causal, tc):
-    if tc and d != 128:
-        pytest.skip("wgmma attention is specialised for head_dim 128")
+def test_attention_fwd(cuda_device, B, T, Hq, Hkv, d, causal):
     from metamorph_b200 import ops
     torch.manual_seed(10)
     qkv = torch.randn(B * T, (Hq + 2 * Hkv) * d, device=cuda_device).bfloat16()
@@ -314,7 +310,7 @@ def test_attention_fwd(cuda_device, B, T, Hq, Hkv, d, causal, tc):
     seqlens = None
     if causal:
         seqlens = torch.tensor([T, max(1, T - 77)][:B], device=cuda_device, dtype=torch.int32)
-    out, lse = ops.attn_fwd(q, k, v, B, T, Hq, Hkv, d, causal, scale, seqlens=seqlens, tc=tc)
+    out, lse = ops.attn_fwd(q, k, v, B, T, Hq, Hkv, d, causal, scale, seqlens=seqlens)
     ref = _attn_ref(q.float().view(B, T, Hq, d), k.float().view(B, T, Hkv, d), v.float().view(B, T, Hkv, d),
                     causal, scale, seqlens)
     o = out.view(B, T, Hq, d).float()
@@ -326,9 +322,8 @@ def test_attention_fwd(cuda_device, B, T, Hq, Hkv, d, causal, tc):
         _close(o, ref, 2e-2, "attn fwd")
 
 
-@pytest.mark.parametrize("tc", [False, True])
 @pytest.mark.parametrize("B,T,Hq,Hkv", [(2, 200, 8, 2), (1, 512, 4, 1), (1, 384, 2, 2), (2, 1501, 8, 2), (1, 2050, 4, 1)])
-def test_attention_bwd(cuda_device, B, T, Hq, Hkv, tc):
+def test_attention_bwd(cuda_device, B, T, Hq, Hkv):
     from metamorph_b200 import ops
     torch.manual_seed(11)
     d = 128
@@ -343,7 +338,7 @@ def test_attention_bwd(cuda_device, B, T, Hq, Hkv, tc):
         dout.view(B, T, -1)[b, int(seqlens[b]):] = 0
     dqkv = torch.zeros_like(qkv)
     ops.attn_bwd(q, k, v, out, dout, lse, dqkv[:, :Hq * d], dqkv[:, Hq * d:(Hq + Hkv) * d],
-                 dqkv[:, (Hq + Hkv) * d:], B, T, Hq, Hkv, d, scale, seqlens=seqlens, tc=tc)
+                 dqkv[:, (Hq + Hkv) * d:], B, T, Hq, Hkv, d, scale, seqlens=seqlens)
     qf = q.float().view(B, T, Hq, d).clone().requires_grad_(True)
     kf = k.float().view(B, T, Hkv, d).clone().requires_grad_(True)
     vf = v.float().view(B, T, Hkv, d).clone().requires_grad_(True)
@@ -355,11 +350,11 @@ def test_attention_bwd(cuda_device, B, T, Hq, Hkv, tc):
         _close(dqkv[:, :Hq * d].view(B, T, Hq, d)[b, :L], qf.grad[b, :L], 3e-2, "dq")
         _close(dqkv[:, Hq * d:(Hq + Hkv) * d].view(B, T, Hkv, d)[b, :L], kf.grad[b, :L], 3e-2, "dk")
         _close(dqkv[:, (Hq + Hkv) * d:].view(B, T, Hkv, d)[b, :L], vf.grad[b, :L], 3e-2, "dv")
-        if tc:      # padded positions are outside the sequence: exactly zero gradients
-            assert float(dqkv.view(B, T, -1)[b, L:].abs().max() if L < T else 0.0) == 0.0
+        # padded positions are outside the sequence: exactly zero gradients
+        assert float(dqkv.view(B, T, -1)[b, L:].abs().max() if L < T else 0.0) == 0.0
 
 
-def test_attention_bwd_tc_ignores_padded_dout_and_is_deterministic(cuda_device):
+def test_attention_bwd_ignores_padded_dout_and_is_deterministic(cuda_device):
     """The wgmma backward treats rows >= seqlens[b] as outside the sequence (the reference's masked positions carry no
     gradient): a non-zero dO there must not change any result; and with no atomics two runs agree bit for bit."""
     from metamorph_b200 import ops
@@ -379,7 +374,7 @@ def test_attention_bwd_tc_ignores_padded_dout_and_is_deterministic(cuda_device):
             do.view(B, T, -1)[1, 300:] = 0
         g = torch.full_like(qkv, float("nan"))
         ops.attn_bwd(q, k, v, out, do, lse, g[:, :Hq * d], g[:, Hq * d:(Hq + Hkv) * d], g[:, (Hq + Hkv) * d:], B, T, Hq,
-                     Hkv, d, scale, seqlens=seqlens, tc=True)
+                     Hkv, d, scale, seqlens=seqlens)
         res.append(g)
     assert torch.equal(res[0], res[1])                        # bit-reproducible
     assert torch.equal(res[0], res[2])                        # dO of the padded rows is ignored
