@@ -20,6 +20,11 @@ def gamma(n, u=U):
     return n * u / (1 - n * u)
 
 
+def expf_fast_rel(arg):
+    """__expf: 2 + floor(1.173 |x|) ulp (CUDA C Programming Guide, intrinsic functions), 1 ulp <= 2u relative."""
+    return (2 + torch.floor(1.173 * arg.abs())) * 2 * U
+
+
 def ints(shape, lo, hi, device, dtype=torch.bfloat16, gen=None):
     return torch.randint(lo, hi + 1, shape, device=device, generator=gen).to(dtype)
 
@@ -115,6 +120,20 @@ def assert_rounds_within(got_bf16, ref64, err64, what):
     assert_between(got_bf16, round_bf16_from_fp64(lo).double(), round_bf16_from_fp64(hi).double(), what)
     r = round_bf16_from_fp64(ref64).double()
     return int(((got_bf16.double() != r) & ~torch.isnan(r)).sum())
+
+
+def rounding_slack(got_bf16, ref64, err64):
+    """How far into its bound a result that passed `assert_rounds_within` went: (the number of elements that differ from
+    round(ref64), the largest |midpoint - ref64| / err64 over them). Such an element's fp32 value lay beyond the midpoint
+    between round(ref64) and the value returned, so the ratio is a lower bound on that element's err / bound."""
+    g, ref64 = got_bf16.double(), ref64.double()
+    err64 = torch.as_tensor(err64, dtype=torch.float64, device=ref64.device).expand_as(ref64)
+    r = round_bf16_from_fp64(ref64).double()
+    off = (g != r) & torch.isfinite(r) & torch.isfinite(g)
+    if not bool(off.any()):
+        return 0, 0.0
+    mid = (g[off] + r[off]) / 2
+    return int(off.sum()), float(((mid - ref64[off]).abs() / err64[off]).max())
 
 
 def err_stats(x, ref):

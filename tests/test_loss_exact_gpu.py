@@ -7,7 +7,8 @@ import numpy as np
 import pytest
 import torch
 
-from tests.exact import U, assert_between, assert_equal, assert_rounds_within, assert_within, gamma, round_bf16_from_fp64
+from tests.exact import (U, assert_between, assert_equal, assert_rounds_within, assert_within, expf_fast_rel, gamma,
+                         round_bf16_from_fp64)
 
 pytestmark = pytest.mark.gpu
 
@@ -22,11 +23,6 @@ def _rnd(x):
     return round_bf16_from_fp64(x).double()
 
 
-def _expf_rel(arg):
-    """__expf: 2 + floor(1.173 |x|) ulp (CUDA C Programming Guide, intrinsic functions); 1 ulp <= 2u relative."""
-    return (2 + torch.floor(1.173 * arg.abs())) * 2 * U
-
-
 # ------------------------------------------------------------------------------------------------ cross-entropy
 # loss.cu:57-124, 256-269: one 512-thread block per row. Pass 1 (online max / sum): thread t takes float4 vectors at
 # 4t, 4t + 2048, ... below V4 = V & ~3 (loss.cu:78-86), then the scalar tail V4 + t < V (loss.cu:87-94); block_max,
@@ -38,7 +34,7 @@ def ce_lse_bound(x, V):
 
     A thread's running sum rescales at most n_it + 1 times (n_it = its vector and tail iterations) and the arguments of
     all its rescales add up to at most W = max - min of the row, so every exp term reaches gs with a relative error of at
-    most 2u (2 (n_it + 2) + 1.7 (W + |x_j - max|)) (__expf as `_expf_rel`, plus u |arg| for each rounded argument);
+    most 2u (2 (n_it + 2) + 1.7 (W + |x_j - max|)) (__expf as `expf_fast_rel`, plus u |arg| for each rounded argument);
     the terms within 40 of the max carry all but e^-40 of the sum, the rest are bounded by their share. The sum adds
     at most gamma_(4 n_it + 10). ln(1 + rho) <= rho; logf is within 1 ulp and gm + log one more rounding."""
     x64 = x.double()
@@ -55,7 +51,7 @@ def ce_lse_bound(x, V):
 def ce_dlogits_ref(x, lse, lse64, labels, gs):
     """fp64 (softmax - onehot) * gs (0 on ignored rows) and the kernel's error before its bf16 rounding. The kernel
     uses its own lse (returned in lse_out), so that error is measured, not bounded: exp(fl(x - lse)) is off by
-    |lse - lse64| + u |arg| + `_expf_rel`(arg) relative; - onehot and * gs round once each.
+    |lse - lse64| + u |arg| + `expf_fast_rel`(arg) relative; - onehot and * gs round once each.
     err = 1.01 gs (p (dlse + u |arg| + e_exp) + u |p - onehot|) + u |ref| + 2^-148."""
     x64 = x.double()
     valid = (labels != -100)[:, None]
@@ -66,7 +62,7 @@ def ce_dlogits_ref(x, lse, lse64, labels, gs):
     ref = (p - oh) * gs * valid
     dlse = (lse.double() - lse64).abs()[:, None]
     arg = x64 - lse.double()[:, None]
-    err = 1.01 * gs * (p * (dlse + U * arg.abs() + _expf_rel(arg)) + U * (p - oh).abs()) + U * ref.abs() + 2.0 ** -148
+    err = 1.01 * gs * (p * (dlse + U * arg.abs() + expf_fast_rel(arg)) + U * (p - oh).abs()) + U * ref.abs() + 2.0 ** -148
     return ref, err * valid
 
 

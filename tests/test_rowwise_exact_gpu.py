@@ -13,7 +13,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from tests.exact import U, assert_between, assert_equal, assert_rounds_within, gamma, round_bf16_from_fp64
+from tests.exact import U, assert_between, assert_equal, assert_rounds_within, expf_fast_rel, gamma, round_bf16_from_fp64
 
 pytestmark = pytest.mark.gpu
 
@@ -319,11 +319,6 @@ def all_bf16(dev):
     return v.to(dev)
 
 
-def expf_fast_rel(arg):
-    """__expf: 2 + floor(1.173 |x|) ulp (CUDA C Programming Guide, intrinsic functions), 1 ulp <= 2u relative."""
-    return (2 + torch.floor(1.173 * arg.abs())) * 2 * U
-
-
 def gelu_ref(x):
     """fp64 erf GELU and the kernel's error. t = fl(x * c32): 2u relative (c32 is 1/sqrt 2 rounded); erf moves by
     erf'(t) |t| 2u; erff is within 2 ulp (<= 4u |erf|); 1 + erf rounds (u |1 + erf|); 0.5 x (...) rounds once more.
@@ -492,3 +487,98 @@ def test_bilinear_l2norm_every_side(cuda_device, S, C, n_img):
         assert_between(y, lo, hi, f"bilinear_l2norm S={S} T={T} C={C}")
     z = ops.bilinear_l2norm(torch.zeros_like(x), 8)
     assert bool((z == 0).all()), "an all-zero feature map must normalise to zeros"
+
+
+# ------------------------------------------------------------------------------------------------ gather / scatter-add rows
+# interleave.cu:126-172, 195-209: grid = min(ceil(R / 8), #SMs * 8) blocks of 8 warps, one row per warp: warp w of block
+# b takes rows b * 8 + w, + grid * 8, ... (a trip covers #SMs * 64 rows once R reaches that); lane l copies or adds the
+# 8-wide vectors l, l + 32, ... of its row. gather_rows is the decode step's last-row pick (engine/decode.py) and the
+# vision-head row selection; scatter_add_rows_ adds the CE and vision-head gradients back into d_hidden
+# (engine/hot_path.py), with unique indices.
+ROW_R = ["1", "sms*64-1", "sms*64", "sms*64+1", "3*sms*64+5"]
+ROW_H = [8, 256, 1152, 4096, 4104]
+
+
+def _row_case(dev, Rk, H):
+    sms = _sms(dev)
+    R = {"1": 1, "sms*64-1": sms * 64 - 1, "sms*64": sms * 64, "sms*64+1": sms * 64 + 1,
+         "3*sms*64+5": 3 * sms * 64 + 5}[Rk]
+    grid = min(-(-R // 8), sms * 8)
+    assert -(-R // (grid * 8)) == {"1": 1, "sms*64-1": 1, "sms*64": 1, "sms*64+1": 2, "3*sms*64+5": 4}[Rk]
+    nvec = H // 8
+    assert (-(-nvec // 32), nvec % 32) == {8: (1, 1), 256: (1, 0), 1152: (5, 16), 4096: (16, 0), 4104: (17, 1)}[H]
+    return R
+
+
+@pytest.mark.parametrize("H", ROW_H)
+@pytest.mark.parametrize("Rk", ROW_R)
+def test_gather_rows_bit_exact_never_reads_unindexed_rows(cuda_device, Rk, H):
+    from metamorph_b200 import ops
+    R = _row_case(cuda_device, Rk, H)
+    Rx = R + 4
+    g = torch.Generator().manual_seed(R + H)
+    x = torch.randn(Rx, H, generator=g).bfloat16()
+    dead = torch.tensor(sorted({1, Rx // 3, Rx // 2, Rx - 2}))
+    x[dead] = float("nan")
+    live = torch.tensor([r for r in range(Rx) if r not in set(dead.tolist())])
+    idx = live.flip(0).repeat(-(-R // live.numel()))[:R].clone()      # reversed, and repeated when R > #live
+    idx[0] = Rx - 1                                                    # the last row
+    if R > 2:
+        idx[2] = idx[1]                                                # a repeated index
+    x, idx = x.to(cuda_device), idx.to(torch.int32).to(cuda_device)
+    buf = torch.full((R + 3, H), float("nan"), dtype=torch.bfloat16, device=cuda_device)
+    guard = buf[R:].clone()
+    ops.gather_rows(x, idx, out=buf[:R])
+    want = x[idx.long()]
+    assert not bool(torch.isnan(want).any())
+    assert_equal(buf[:R], want, f"gather_rows R={R} H={H}")
+    assert torch.equal(buf[R:].view(torch.int16), guard.view(torch.int16)), "guard rows after out were written"
+
+
+@pytest.mark.parametrize("H", ROW_H)
+@pytest.mark.parametrize("Rk", ROW_R)
+def test_scatter_add_rows_rounds_like_fp64(cuda_device, Rk, H):
+    """x[idx[i]] = bf16(x[idx[i]] + g[i]) in fp32, which is bit-equal to the single rounding of the exact sum: two bf16
+    values whose exponents differ by at most 16 add exactly in fp32 (8 + 16 significant bits fit in 24); otherwise the
+    smaller is below 2^-16 of the larger, and both the exact and the fp32 sum lie within 2^-16 (relative) of the larger,
+    a bf16 value, whose neighbouring bf16 midpoints are at least 2^-10 away: both round to it. Overflow and ±inf agree
+    too (the sum past bf16's largest finite value rounds to inf either way; inf + -inf is NaN)."""
+    from metamorph_b200 import ops
+    R = _row_case(cuda_device, Rk, H)
+    Rx = R + 4
+    g = torch.Generator().manual_seed(3 * R + H)
+    idx = torch.randperm(Rx, generator=g)[:R]                          # unique, in no order
+    x = torch.full((Rx, H), float("nan"))
+    x[idx] = torch.randn(R, H, generator=g) * torch.pow(2.0, torch.randint(-24, 25, (R, H), generator=g).float())
+    gr = torch.randn(R, H, generator=g) * torch.pow(2.0, torch.randint(-24, 25, (R, H), generator=g).float())
+    r0 = int(idx[0])
+    x[r0, :6] = torch.tensor([float("inf"), float("-inf"), 3e38, -3e38, float("inf"), 1.0])
+    gr[0, :6] = torch.tensor([1.0, -2.0, 3e38, -3e38, float("-inf"), float("inf")])
+    x, gr = x.bfloat16(), gr.bfloat16()
+    x, gr, idx = x.to(cuda_device), gr.to(cuda_device), idx.to(torch.int32).to(cuda_device)
+    x0 = x.clone()
+    ops.scatter_add_rows_(x, idx, gr)
+    il = idx.long()
+    exact = x0[il].double() + gr.double()
+    sp = round_bf16_from_fp64(exact[0, :6]).float()                    # ±inf, overflow to ±inf, inf - inf
+    assert bool(torch.isposinf(sp[[0, 2, 5]]).all()) and bool(torch.isneginf(sp[[1, 3]]).all())
+    assert bool(torch.isnan(sp[4])) and bool(torch.isfinite(exact[0, 2:4]).all())
+    assert_rounds_within(x[il], exact, 0.0, f"scatter_add_rows_ R={R} H={H}")
+    rest = torch.ones(Rx, dtype=torch.bool, device=cuda_device)
+    rest[il] = False
+    assert torch.equal(x[rest].view(torch.int16), x0[rest].view(torch.int16)), "a row not in idx was written"
+
+
+def test_row_kernels_refuse_h_not_multiple_of_8(cuda_device):
+    from metamorph_b200 import ops
+    from metamorph_b200._lib import MetaMorphB200Error
+    x = torch.randn(4, 12, device=cuda_device).bfloat16()
+    idx = torch.tensor([3, 0], dtype=torch.int32, device=cuda_device)
+    out = torch.full((2, 12), float("nan"), dtype=torch.bfloat16, device=cuda_device)
+    x0 = x.clone()
+    with pytest.raises(MetaMorphB200Error, match="H%8"):
+        ops.gather_rows(x, idx, out=out)
+    with pytest.raises(MetaMorphB200Error, match="H%8"):
+        ops.scatter_add_rows_(x, idx, torch.ones(2, 12, dtype=torch.bfloat16, device=cuda_device))
+    torch.cuda.synchronize()
+    assert bool(torch.isnan(out).all()) and torch.equal(x, x0), "a refused call wrote its output"
