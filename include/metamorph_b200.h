@@ -230,6 +230,35 @@ int mm_kv_prefill_paged(const void* qkv, long long ld, void* kpool, void* vpool,
 int mm_attn_fwd_tc_paged(const void* q, long long ldq, const void* kpool, const void* vpool, int num_blocks,
                          const int* block_table_row, int max_blocks, int block_size, void* o, long long ldo,
                          int q_start, int n_q, int Hq, int Hkv, int head_dim, float scale, cudaStream_t s);
+/* FP8 KV cache (E4M3). Each (position, kv head) row of 128 values x is stored as q_i = RNE_e4m3(x_i 2^-e) with one fp32
+ * scale 2^e: a = max |x_i|, e the least integer with a <= 448 2^e, at least -124; a zero row stores zeros with e = 0, a
+ * row holding Inf or NaN stores 0x7f (E4M3 NaN) everywhere with e = 0; at e = 120 an entry that rounds to 256 (|x| >=
+ * 1.9375 2^127, whose x-hat 2^128 would overflow) stores 240 instead. x-hat_i = float(q_i) 2^e is exact and a bf16
+ * value. A row's bytes depend on that row alone. Byte caches are the bf16 layouts above; scales are addressed like the
+ * rows: [B, Hkv, Tmax] dense, [num_blocks, Hkv, block_size] paged (scale index = element offset of the row / 128).
+ * mm_decode_attn_fp8 / mm_decode_attn_paged_fp8: mm_decode_attn / mm_decode_attn_paged on such a cache. The owner of pos
+ * quantises the rotated new k and the new v, appends bytes and scales and scores pos from their x-hat; with equal splits
+ * the output bits are those of the bf16 call on a bf16 cache holding x-hat (appended rows included).
+ * mm_kv_quant_prefill[_paged]: mm_kv_prefill[_paged] for such a cache; also overwrites the K and V columns of qkv with
+ * x-hat (Q columns untouched), so a prefill's attention reads what the cache holds. qkv rows must be 8-byte aligned.
+ * mm_kv_dequant_paged: staging block i <- x-hat of pool block block_table_row[i] for i < n_blocks, into bf16 staging
+ * pools [>= n_blocks, Hkv, block_size, 128]. Every scale pointer must be non-null. */
+int mm_decode_attn_fp8(const void* qkv, long long ldqkv, void* kcache, void* vcache, float* kscale, float* vscale,
+                       const int* pos, const float* cos_t, const float* sin_t, void* out, long long ldo, int B, int Hq,
+                       int Hkv, int head_dim, int Tmax, float scale, void* workspace, long long workspace_bytes,
+                       int splits, cudaStream_t s);
+int mm_decode_attn_paged_fp8(const void* qkv, long long ldqkv, void* kpool, void* vpool, float* kscale, float* vscale,
+                             const int* block_table, int max_blocks, int block_size, const int* pos, const float* cos_t,
+                             const float* sin_t, void* out, long long ldo, int B, int Hq, int Hkv, int head_dim,
+                             float scale, void* workspace, long long workspace_bytes, int splits, cudaStream_t s);
+int mm_kv_quant_prefill(void* qkv, long long ld, void* kcache, void* vcache, float* kscale, float* vscale, int B, int T,
+                        int Hq, int Hkv, int head_dim, int Tmax, cudaStream_t s);
+int mm_kv_quant_prefill_paged(void* qkv, long long ld, void* kpool, void* vpool, float* kscale, float* vscale,
+                              const int* block_table_row, int max_blocks, int block_size, int T, int Hq, int Hkv,
+                              int head_dim, cudaStream_t s);
+int mm_kv_dequant_paged(const void* kpool, const void* vpool, const float* kscale, const float* vscale,
+                        const int* block_table_row, int max_blocks, int block_size, int n_blocks, int Hkv,
+                        int head_dim, void* kstage, void* vstage, cudaStream_t s);
 int mm_decode_state_step(int* in_image_mode, int* total_image_tokens, int* total_output, int* finished, int* pos,
                          int* n_ids, int* n_img, int* ids_out, int* append_kind, int* next_token,
                          const int* argmax_tok, const int* forced, int forced_ld, int step, int B,

@@ -55,7 +55,7 @@ def ll(x) -> c_longlong:
 
 # kernels launched per C-ABI call (for bench.py's `gpu_launches` claim); default 1
 _LAUNCHES = {"mm_attn_bwd_tc": 2, "mm_attn_bwd_tc_varlen": 2, "mm_clip_coef": 1, "mm_decode_attn": 2,
-             "mm_decode_attn_paged": 2, "mm_sumsq_bf16_accum": 2}
+             "mm_decode_attn_paged": 2, "mm_decode_attn_fp8": 2, "mm_decode_attn_paged_fp8": 2, "mm_sumsq_bf16_accum": 2}
 launch_count = 0
 
 

@@ -13,7 +13,9 @@
 //   decode_state  the per-sequence text/image mode state machine of greedy_decode
 //                 (metamorph_llama.py:547-582) on the device: no .item() host syncs.
 #include "common.cuh"
+#include <cuda_fp8.h>
 #include <mutex>
+#include <type_traits>
 #include <stdlib.h>
 
 typedef CUresult (*PFN_encodeTiledSk)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -204,16 +206,78 @@ skinny_gemm_tma_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
 // address of a K/V row changes: the split, the walk order and the arithmetic are the dense kernel's, so both give the
 // same bits on the same logical cache. The table row is read through the read-only path (one entry per position, L1
 // resident), which leaves the shared-memory footprint of the dense kernel unchanged.
+// FP8: K/V rows are E4M3 bytes with one fp32 power-of-two scale per (position, kv head) row (fp8_quant_row_warp); the
+// scale arrays are addressed like the rows ([B, Hkv, Tmax] dense, [num_blocks, Hkv, block_size] paged). Every cached
+// element is dequantised to float(q) * 2^e, an exact bf16 value, and then meets the bf16 kernel's arithmetic unchanged,
+// so the output bits are the bf16 kernel's on a bf16 cache holding those values. The owner of pos quantises the new
+// k / v, appends them and scores pos from the dequantised copies.
 constexpr int DA_THREADS = 256;
 constexpr int DA_D = 128;
 
-template <int G, bool PAGED>
+// E4M3 row quantisation, one warp per 128-value row, 4 values per lane (any assignment of values to lanes). a = max |x|;
+// e = the least integer with a <= 448 * 2^e, at least -124 (so every float(q) * 2^e is a bf16 value and 2^e an fp32
+// normal); q = RNE_e4m3(x * 2^-e) (exact multiply, |x * 2^-e| <= 448: nothing saturates), except that at e = 120, the
+// largest e a bf16 row reaches, an entry that rounds to 256 (|x| >= 1.9375 * 2^127) would dequantise to 2^128, past the
+// bf16 and fp32 range: it stores 240 (0x77), the largest magnitude whose float(q) * 2^e is finite. A zero row stores
+// zeros with e = 0; a row holding any Inf or NaN stores the E4M3 NaN 0x7f everywhere with e = 0. On return x holds
+// float(q) * 2^e, q01 / q23 the bytes of (x[0], x[1]) and (x[2], x[3]) (first value in the low byte); returns 2^e.
+__device__ __forceinline__ uint16_t fp8x2_cap_256(uint16_t q) {
+  const uint16_t lo = (q & 0x7f) == 0x78 ? (q & 0x80) | 0x77 : q & 0xff;
+  const uint16_t hi = ((q >> 8) & 0x7f) == 0x78 ? ((q >> 8) & 0x80) | 0x77 : q >> 8;
+  return (uint16_t)(lo | (hi << 8));
+}
+
+__device__ __forceinline__ float fp8_quant_row_warp(float (&x)[4], uint16_t& q01, uint16_t& q23) {
+  float a = 0.f;
+  bool bad = false;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float m = fabsf(x[j]);
+    bad |= !(m <= 3.402823466e38f);
+    a = fmaxf(a, m);
+  }
+  a = warp_max(a);
+  bad = __any_sync(0xffffffffu, bad);
+  int e = 0;
+  if (!bad && a > 0.f) {
+    int E;
+    const float f = frexpf(a, &E);          // a = f 2^E, f in [0.5, 1); 448 = 0.875 * 2^9
+    e = max(f <= 0.875f ? E - 9 : E - 8, -124);
+  }
+  const float sc = __int_as_float((127 + e) << 23), inv = __int_as_float((127 - e) << 23);
+  if (bad) {
+    q01 = q23 = 0x7f7f;
+  } else {
+    q01 = __nv_cvt_float2_to_fp8x2(make_float2(x[0] * inv, x[1] * inv), __NV_SATFINITE, __NV_E4M3);
+    q23 = __nv_cvt_float2_to_fp8x2(make_float2(x[2] * inv, x[3] * inv), __NV_SATFINITE, __NV_E4M3);
+    if (e == 120) {
+      q01 = fp8x2_cap_256(q01);
+      q23 = fp8x2_cap_256(q23);
+    }
+  }
+  const float2 d01 = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2(q01, __NV_E4M3)));
+  const float2 d23 = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2(q23, __NV_E4M3)));
+  x[0] = d01.x * sc; x[1] = d01.y * sc; x[2] = d23.x * sc; x[3] = d23.y * sc;
+  return sc;
+}
+
+// four E4M3 values (first in the low byte) -> float(q) * sc
+__device__ __forceinline__ void fp8x4_dequant(uint32_t u, float sc, float* f) {
+  const float2 a = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(u & 0xffffu), __NV_E4M3)));
+  const float2 b = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(u >> 16), __NV_E4M3)));
+  f[0] = a.x * sc; f[1] = a.y * sc; f[2] = b.x * sc; f[3] = b.y * sc;
+}
+
+template <int G, bool PAGED, bool FP8 = false>
 __global__ void __launch_bounds__(DA_THREADS)
-decode_attn_kernel(const bf16* __restrict__ qkv, long long ldqkv, bf16* __restrict__ kc,
-                   bf16* __restrict__ vc, const int* __restrict__ pos_arr,
+decode_attn_kernel(const bf16* __restrict__ qkv, long long ldqkv,
+                   std::conditional_t<FP8, uint8_t, bf16>* __restrict__ kc,
+                   std::conditional_t<FP8, uint8_t, bf16>* __restrict__ vc, const int* __restrict__ pos_arr,
                    const float* __restrict__ cos_t, const float* __restrict__ sin_t,
                    float* __restrict__ part, int Hq, int Hkv, int Tmax, int S, float scale,
-                   const int* __restrict__ table, int max_blocks, int bs_shift) {
+                   const int* __restrict__ table, int max_blocks, int bs_shift, float* __restrict__ ksc,
+                   float* __restrict__ vsc) {
+  using KVT = std::conditional_t<FP8, uint8_t, bf16>;
   extern __shared__ float sm[];
   float* sq = sm;                          // [G][128] rotated, scaled q
   float* sknew = sq + G * DA_D;            // [128] rotated new k
@@ -230,8 +294,8 @@ decode_attn_kernel(const bf16* __restrict__ qkv, long long ldqkv, bf16* __restri
   const int cpad = ((Tmax + S - 1) / S + 4) & ~3;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const bf16* row = qkv + (long long)b * ldqkv;
-  bf16* kcb = kc + (PAGED ? 0ll : ((long long)b * Hkv + hk) * Tmax * DA_D);
-  bf16* vcb = vc + (PAGED ? 0ll : ((long long)b * Hkv + hk) * Tmax * DA_D);
+  KVT* kcb = kc + (PAGED ? 0ll : ((long long)b * Hkv + hk) * Tmax * DA_D);
+  KVT* vcb = vc + (PAGED ? 0ll : ((long long)b * Hkv + hk) * Tmax * DA_D);
   const int* trow = PAGED ? table + (long long)b * max_blocks : nullptr;
   // element offset of the K/V row of logical position p, relative to kcb / vcb
   auto row_off = [&](int p) -> long long {
@@ -242,6 +306,17 @@ decode_attn_kernel(const bf16* __restrict__ qkv, long long ldqkv, bf16* __restri
       return (long long)p * DA_D;
     }
   };
+  // FP8: index of the row of p (row_off(p) / 128) in the scale arrays, relative to kscb / vscb
+  auto row_idx = [&](int p) -> long long {
+    if constexpr (PAGED) {
+      const long long blk = __ldg(trow + (p >> bs_shift));
+      return ((blk * Hkv + hk) << bs_shift) + (p & ((1 << bs_shift) - 1));
+    } else {
+      return (long long)p;
+    }
+  };
+  float* kscb = FP8 ? ksc + (PAGED ? 0ll : ((long long)b * Hkv + hk) * Tmax) : nullptr;
+  float* vscb = FP8 ? vsc + (PAGED ? 0ll : ((long long)b * Hkv + hk) * Tmax) : nullptr;
   const float* cp = cos_t + (long long)pos * (DA_D / 2);
   const float* sp_ = sin_t + (long long)pos * (DA_D / 2);
   const bool owns_new = (pos >= p0 && pos < p1);
@@ -253,7 +328,42 @@ decode_attn_kernel(const bf16* __restrict__ qkv, long long ldqkv, bf16* __restri
     sq[h * DA_D + j] = __bfloat162float(__float2bfloat16(rope_lo(a, c, cp[j], sp_[j]))) * scale;
     sq[h * DA_D + j + DA_D / 2] = __bfloat162float(__float2bfloat16(rope_hi(a, c, cp[j], sp_[j]))) * scale;
   }
-  if (owns_new && tid < DA_D / 2) {
+  if constexpr (FP8) {
+    // warp 0 quantises the rotated new k (lane: dims 2l, 2l+1, 2l+64, 2l+65), warp 1 the new v (dims 4l .. 4l+3)
+    if (owns_new && warp < 2) {
+      const long long ri = row_idx(pos);
+      float x[4];
+      if (warp == 0) {
+        const bf16* kh = row + (long long)(Hq + hk) * DA_D;
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const int j = 2 * lane + u;
+          const float a = __bfloat162float(kh[j]), c = __bfloat162float(kh[j + DA_D / 2]);
+          x[u] = __bfloat162float(__float2bfloat16(rope_lo(a, c, cp[j], sp_[j])));
+          x[2 + u] = __bfloat162float(__float2bfloat16(rope_hi(a, c, cp[j], sp_[j])));
+        }
+        uint16_t q01, q23;
+        const float sc = fp8_quant_row_warp(x, q01, q23);
+        *reinterpret_cast<uint16_t*>(kcb + ri * DA_D + 2 * lane) = q01;
+        *reinterpret_cast<uint16_t*>(kcb + ri * DA_D + DA_D / 2 + 2 * lane) = q23;
+        if (lane == 0) kscb[ri] = sc;
+        sknew[2 * lane] = x[0];
+        sknew[2 * lane + 1] = x[1];
+        sknew[DA_D / 2 + 2 * lane] = x[2];
+        sknew[DA_D / 2 + 2 * lane + 1] = x[3];
+      } else {
+        const uint2 raw = *reinterpret_cast<const uint2*>(row + (long long)(Hq + Hkv + hk) * DA_D + 4 * lane);
+        const float2 f0 = unpack_bf16x2(raw.x), f1 = unpack_bf16x2(raw.y);
+        x[0] = f0.x; x[1] = f0.y; x[2] = f1.x; x[3] = f1.y;
+        uint16_t q01, q23;
+        const float sc = fp8_quant_row_warp(x, q01, q23);
+        *reinterpret_cast<uint32_t*>(vcb + ri * DA_D + 4 * lane) = (uint32_t)q01 | ((uint32_t)q23 << 16);
+        if (lane == 0) vscb[ri] = sc;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) svnew[4 * lane + j] = x[j];
+      }
+    }
+  } else if (owns_new && tid < DA_D / 2) {
     const bf16* kh = row + (long long)(Hq + hk) * DA_D;
     const bf16* vh = row + (long long)(Hq + Hkv + hk) * DA_D;
     const float a = __bfloat162float(kh[tid]), c = __bfloat162float(kh[tid + DA_D / 2]);
@@ -281,6 +391,34 @@ decode_attn_kernel(const bf16* __restrict__ qkv, long long ldqkv, bf16* __restri
         const float kf = sknew[d];
 #pragma unroll
         for (int h = 0; h < G; ++h) s[h] += sq[h * DA_D + d] * kf;
+      }
+    } else if constexpr (FP8) {
+      // the whole 128 B row is requested at once (8 x 16 B); each 16 B feeds two of the bf16 kernel's 8-value
+      // groups, in the same order
+      const long long ri = row_idx(p);
+      const int4* kp = reinterpret_cast<const int4*>(kcb + ri * DA_D);
+      const float ks = kscb[ri];
+      int4 rawk[DA_D / 16];
+#pragma unroll
+      for (int v2 = 0; v2 < DA_D / 16; ++v2) rawk[v2] = kp[v2];
+#pragma unroll
+      for (int v2 = 0; v2 < DA_D / 16; ++v2) {
+        const int4 raw = rawk[v2];
+        const uint32_t u[4] = {(uint32_t)raw.x, (uint32_t)raw.y, (uint32_t)raw.z, (uint32_t)raw.w};
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          const int v = 2 * v2 + half;
+          float kf[8];
+          fp8x4_dequant(u[2 * half], ks, kf);
+          fp8x4_dequant(u[2 * half + 1], ks, kf + 4);
+#pragma unroll
+          for (int h = 0; h < G; ++h) {
+            const float4 q0 = *reinterpret_cast<const float4*>(sq + h * DA_D + v * 8);
+            const float4 q1 = *reinterpret_cast<const float4*>(sq + h * DA_D + v * 8 + 4);
+            s[h] += q0.x * kf[0] + q0.y * kf[1] + q0.z * kf[2] + q0.w * kf[3] + q1.x * kf[4] + q1.y * kf[5] +
+                    q1.z * kf[6] + q1.w * kf[7];
+          }
+        }
       }
     } else {
       const int4* kp = reinterpret_cast<const int4*>(kcb + row_off(p));
@@ -342,6 +480,9 @@ decode_attn_kernel(const bf16* __restrict__ qkv, long long ldqkv, bf16* __restri
         if (p == pos) {
 #pragma unroll
           for (int j = 0; j < 4; ++j) vf[u][j] = svnew[lane * 4 + j];
+        } else if constexpr (FP8) {
+          const long long ri = row_idx(p);
+          fp8x4_dequant(*reinterpret_cast<const uint32_t*>(vcb + ri * DA_D + lane * 4), vscb[ri], vf[u]);
         } else {
           const uint2 raw = *reinterpret_cast<const uint2*>(vcb + row_off(p) + lane * 4);
           const float2 f0 = unpack_bf16x2(raw.x), f1 = unpack_bf16x2(raw.y);
@@ -439,6 +580,79 @@ __global__ void kv_prefill_paged_kernel(const bf16* __restrict__ qkv, long long 
     const long long dst = (((blk * Hkv + hk) << bs_shift) + (t & ((1 << bs_shift) - 1))) * DA_D + v * 8;
     *reinterpret_cast<int4*>(kc + dst) = *reinterpret_cast<const int4*>(src + (long long)(Hq + hk) * DA_D + v * 8);
     *reinterpret_cast<int4*>(vc + dst) = *reinterpret_cast<const int4*>(src + (long long)(Hq + Hkv + hk) * DA_D + v * 8);
+  }
+}
+
+// FP8 prefill: quantise the post-RoPE K and V rows of qkv rows [B*T, ld] (one warp per row, fp8_quant_row_warp) into the
+// cache, and overwrite qkv's K / V columns with the dequantised rows, so that the prefill's attention reads exactly the
+// values the cache holds. Dense: bytes [B, Hkv, Tmax, 128], scales [B, Hkv, Tmax]. PAGED (one sequence, B = 1): pools
+// [num_blocks, Hkv, 1 << bs_shift, 128] and scales [num_blocks, Hkv, 1 << bs_shift] through the table row trow.
+template <bool PAGED>
+__global__ void kv_quant_prefill_kernel(bf16* __restrict__ qkv, long long ld, uint8_t* __restrict__ kc,
+                                        uint8_t* __restrict__ vc, float* __restrict__ ks, float* __restrict__ vs,
+                                        const int* __restrict__ trow, int B, int T, int Hq, int Hkv, int Tmax,
+                                        int bs_shift) {
+  const int lane = threadIdx.x & 31;
+  const long long total = (long long)B * T * Hkv * 2;
+  const long long stride = ((long long)gridDim.x * blockDim.x) >> 5;
+  for (long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < total; w += stride) {
+    const int kind = (int)(w & 1);          // 0: K, 1: V
+    long long r = w >> 1;
+    const int hk = (int)(r % Hkv);
+    r /= Hkv;
+    const int t = (int)(r % T), b = (int)(r / T);
+    bf16* src = qkv + ((long long)b * T + t) * ld + (long long)(Hq + kind * Hkv + hk) * DA_D + 4 * lane;
+    long long ri;
+    if constexpr (PAGED) {
+      const long long blk = __ldg(trow + (t >> bs_shift));
+      ri = ((blk * Hkv + hk) << bs_shift) + (t & ((1 << bs_shift) - 1));
+    } else {
+      ri = ((long long)b * Hkv + hk) * Tmax + t;
+    }
+    const uint2 raw = *reinterpret_cast<const uint2*>(src);
+    const float2 f0 = unpack_bf16x2(raw.x), f1 = unpack_bf16x2(raw.y);
+    float x[4] = {f0.x, f0.y, f1.x, f1.y};
+    uint16_t q01, q23;
+    const float sc = fp8_quant_row_warp(x, q01, q23);
+    *reinterpret_cast<uint32_t*>((kind ? vc : kc) + ri * DA_D + 4 * lane) = (uint32_t)q01 | ((uint32_t)q23 << 16);
+    if (lane == 0) (kind ? vs : ks)[ri] = sc;
+    const __nv_bfloat162 h01 = __floats2bfloat162_rn(x[0], x[1]), h23 = __floats2bfloat162_rn(x[2], x[3]);
+    uint2 out;
+    out.x = *reinterpret_cast<const uint32_t*>(&h01);
+    out.y = *reinterpret_cast<const uint32_t*>(&h23);
+    *reinterpret_cast<uint2*>(src) = out;
+  }
+}
+
+// bf16 staging copy of an FP8 pool: staging block i <- float(q) * 2^e of pool block trow[i], i < n_blocks (K and V)
+__global__ void kv_dequant_paged_kernel(const uint8_t* __restrict__ kp, const uint8_t* __restrict__ vp,
+                                        const float* __restrict__ ks, const float* __restrict__ vs,
+                                        const int* __restrict__ trow, int n_blocks, int Hkv, int bs_shift,
+                                        bf16* __restrict__ kst, bf16* __restrict__ vst) {
+  const long long per_blk = (long long)Hkv << bs_shift;   // rows of one block
+  const long long rows = n_blocks * per_blk;
+  const long long total = rows * (DA_D / 16) * 2;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % (DA_D / 16));
+    const long long r = (i / (DA_D / 16)) % rows;
+    const int kind = (int)(i / ((DA_D / 16) * rows));
+    const long long src_row = (long long)__ldg(trow + r / per_blk) * per_blk + r % per_blk;
+    const int4 raw = reinterpret_cast<const int4*>((kind ? vp : kp) + src_row * DA_D)[c];
+    const float sc = (kind ? vs : ks)[src_row];
+    const uint32_t u[4] = {(uint32_t)raw.x, (uint32_t)raw.y, (uint32_t)raw.z, (uint32_t)raw.w};
+    uint32_t o[8];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      float f[4];
+      fp8x4_dequant(u[j], sc, f);
+      const __nv_bfloat162 a = __floats2bfloat162_rn(f[0], f[1]), b = __floats2bfloat162_rn(f[2], f[3]);
+      o[2 * j] = *reinterpret_cast<const uint32_t*>(&a);
+      o[2 * j + 1] = *reinterpret_cast<const uint32_t*>(&b);
+    }
+    int4* dst = reinterpret_cast<int4*>((kind ? vst : kst) + r * DA_D + c * 16);
+    dst[0] = make_int4((int)o[0], (int)o[1], (int)o[2], (int)o[3]);
+    dst[1] = make_int4((int)o[4], (int)o[5], (int)o[6], (int)o[7]);
   }
 }
 
@@ -632,11 +846,14 @@ MM_API long long mm_decode_attn_workspace_bytes(int B, int Hq, int Hkv, int spli
 namespace {
 
 // shared by the dense and the paged entry points; `name` prefixes the error messages. Dense: table == nullptr.
-template <bool PAGED>
+template <bool PAGED, bool FP8 = false>
 int decode_attn_launch(const char* name, const void* qkv, long long ldqkv, void* kcache, void* vcache, const int* pos,
                        const float* cos_t, const float* sin_t, void* out, long long ldo, int B, int Hq, int Hkv,
                        int head_dim, int Tmax, float scale, void* workspace, long long workspace_bytes, int splits,
-                       const int* table, int max_blocks, int bs_shift, cudaStream_t stream) {
+                       const int* table, int max_blocks, int bs_shift, cudaStream_t stream, float* kscale = nullptr,
+                       float* vscale = nullptr) {
+  using KVT = std::conditional_t<FP8, uint8_t, bf16>;
+  MM_CHECK_ARG(!FP8 || (kscale != nullptr && vscale != nullptr), "%s: scale arrays missing", name);
   MM_CHECK_ARG(head_dim == DA_D && Hq % Hkv == 0, "%s: need head_dim 128", name);
   const int G = Hq / Hkv;
   MM_CHECK_ARG(G == 1 || G == 2 || G == 4 || G == 8, "%s: GQA group must be 1, 2, 4 or 8", name);
@@ -650,11 +867,12 @@ int decode_attn_launch(const char* name, const void* qkv, long long ldqkv, void*
 #define MM_DA_LAUNCH(GG)                                                                                     \
   do {                                                                                                       \
     if (smem > 48 * 1024)                                                                                    \
-      MM_CHECK_CUDA(cudaFuncSetAttribute(decode_attn_kernel<GG, PAGED>,                                      \
+      MM_CHECK_CUDA(cudaFuncSetAttribute(decode_attn_kernel<GG, PAGED, FP8>,                                 \
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));           \
-    MM_CHECK_CUDA(launch_pdl(decode_attn_kernel<GG, PAGED>, grid, dim3(DA_THREADS), smem, stream,            \
-                             (const bf16*)qkv, ldqkv, (bf16*)kcache, (bf16*)vcache, pos, cos_t, sin_t,       \
-                             (float*)workspace, Hq, Hkv, Tmax, splits, scale, table, max_blocks, bs_shift));  \
+    MM_CHECK_CUDA(launch_pdl(decode_attn_kernel<GG, PAGED, FP8>, grid, dim3(DA_THREADS), smem, stream,       \
+                             (const bf16*)qkv, ldqkv, (KVT*)kcache, (KVT*)vcache, pos, cos_t, sin_t,         \
+                             (float*)workspace, Hq, Hkv, Tmax, splits, scale, table, max_blocks, bs_shift,   \
+                             kscale, vscale));                                                               \
   } while (0)
   if (G == 1) MM_DA_LAUNCH(1);
   else if (G == 2) MM_DA_LAUNCH(2);
@@ -699,6 +917,97 @@ MM_API int mm_decode_attn_paged(const void* qkv, long long ldqkv, void* kpool, v
   return decode_attn_launch<true>("mm_decode_attn_paged", qkv, ldqkv, kpool, vpool, pos, cos_t, sin_t, out, ldo, B,
                                   Hq, Hkv, head_dim, max_blocks * block_size, scale, workspace, workspace_bytes,
                                   splits, block_table, max_blocks, shift, stream);
+}
+
+MM_API int mm_decode_attn_fp8(const void* qkv, long long ldqkv, void* kcache, void* vcache, float* kscale,
+                              float* vscale, const int* pos, const float* cos_t, const float* sin_t, void* out,
+                              long long ldo, int B, int Hq, int Hkv, int head_dim, int Tmax, float scale,
+                              void* workspace, long long workspace_bytes, int splits, cudaStream_t stream) {
+  return decode_attn_launch<false, true>("mm_decode_attn_fp8", qkv, ldqkv, kcache, vcache, pos, cos_t, sin_t, out, ldo,
+                                         B, Hq, Hkv, head_dim, Tmax, scale, workspace, workspace_bytes, splits, nullptr,
+                                         0, 0, stream, kscale, vscale);
+}
+
+MM_API int mm_decode_attn_paged_fp8(const void* qkv, long long ldqkv, void* kpool, void* vpool, float* kscale,
+                                    float* vscale, const int* block_table, int max_blocks, int block_size,
+                                    const int* pos, const float* cos_t, const float* sin_t, void* out, long long ldo,
+                                    int B, int Hq, int Hkv, int head_dim, float scale, void* workspace,
+                                    long long workspace_bytes, int splits, cudaStream_t stream) {
+  const int shift = paged_block_shift(block_size);
+  MM_CHECK_ARG(shift >= 0, "mm_decode_attn_paged_fp8: block_size must be a power of two in [16,256] (got %d)",
+               block_size);
+  MM_CHECK_ARG(max_blocks >= 1, "mm_decode_attn_paged_fp8: max_blocks must be >= 1 (got %d)", max_blocks);
+  MM_CHECK_ARG(block_table != nullptr, "mm_decode_attn_paged_fp8: block table missing");
+  MM_CHECK_ARG(Hkv >= 1, "mm_decode_attn_paged_fp8: need Hkv >= 1");
+  MM_CHECK_ARG((long long)max_blocks * block_size <= (1 << 30), "mm_decode_attn_paged_fp8: max_blocks too large");
+  return decode_attn_launch<true, true>("mm_decode_attn_paged_fp8", qkv, ldqkv, kpool, vpool, pos, cos_t, sin_t, out,
+                                        ldo, B, Hq, Hkv, head_dim, max_blocks * block_size, scale, workspace,
+                                        workspace_bytes, splits, block_table, max_blocks, shift, stream, kscale, vscale);
+}
+
+namespace {
+
+int kv_quant_prefill_launch(const char* name, void* qkv, long long ld, void* kc, void* vc, float* ks, float* vs,
+                            const int* trow, int B, int T, int Hq, int Hkv, int head_dim, int Tmax, int shift,
+                            cudaStream_t stream) {
+  MM_CHECK_ARG(ks != nullptr && vs != nullptr, "%s: scale arrays missing", name);
+  MM_CHECK_ARG(head_dim == DA_D && Hkv >= 1 && B >= 1 && T >= 0, "%s: need head_dim 128, Hkv >= 1, B >= 1, T >= 0",
+               name);
+  MM_CHECK_ARG(ld % 4 == 0 && ((uintptr_t)qkv & 7) == 0, "%s: qkv rows must be 8-byte aligned", name);
+  if (T == 0) return MM_OK;
+  const long long total = (long long)B * T * Hkv * 2 * 32;
+  long long blocks = ceil_div64(total, 256);
+  if (blocks > (long long)mm_num_sms() * 16) blocks = (long long)mm_num_sms() * 16;
+  if (trow)
+    kv_quant_prefill_kernel<true><<<(int)blocks, 256, 0, stream>>>((bf16*)qkv, ld, (uint8_t*)kc, (uint8_t*)vc, ks, vs,
+                                                                   trow, B, T, Hq, Hkv, Tmax, shift);
+  else
+    kv_quant_prefill_kernel<false><<<(int)blocks, 256, 0, stream>>>((bf16*)qkv, ld, (uint8_t*)kc, (uint8_t*)vc, ks, vs,
+                                                                    nullptr, B, T, Hq, Hkv, Tmax, 0);
+  MM_CHECK_LAUNCH();
+  return MM_OK;
+}
+
+}  // namespace
+
+MM_API int mm_kv_quant_prefill(void* qkv, long long ld, void* kcache, void* vcache, float* kscale, float* vscale, int B,
+                               int T, int Hq, int Hkv, int head_dim, int Tmax, cudaStream_t stream) {
+  MM_CHECK_ARG(T <= Tmax, "mm_kv_quant_prefill: need T <= Tmax");
+  return kv_quant_prefill_launch("mm_kv_quant_prefill", qkv, ld, kcache, vcache, kscale, vscale, nullptr, B, T, Hq, Hkv,
+                                 head_dim, Tmax, 0, stream);
+}
+
+MM_API int mm_kv_quant_prefill_paged(void* qkv, long long ld, void* kpool, void* vpool, float* kscale, float* vscale,
+                                     const int* block_table_row, int max_blocks, int block_size, int T, int Hq,
+                                     int Hkv, int head_dim, cudaStream_t stream) {
+  const int shift = paged_block_shift(block_size);
+  MM_CHECK_ARG(shift >= 0, "mm_kv_quant_prefill_paged: block_size must be a power of two in [16,256] (got %d)",
+               block_size);
+  MM_CHECK_ARG(max_blocks >= 1, "mm_kv_quant_prefill_paged: max_blocks must be >= 1 (got %d)", max_blocks);
+  MM_CHECK_ARG(block_table_row != nullptr, "mm_kv_quant_prefill_paged: block table missing");
+  MM_CHECK_ARG((long long)T <= (long long)max_blocks * block_size, "mm_kv_quant_prefill_paged: need T <= max_blocks * block_size");
+  return kv_quant_prefill_launch("mm_kv_quant_prefill_paged", qkv, ld, kpool, vpool, kscale, vscale, block_table_row, 1,
+                                 T, Hq, Hkv, head_dim, 0, shift, stream);
+}
+
+MM_API int mm_kv_dequant_paged(const void* kpool, const void* vpool, const float* kscale, const float* vscale,
+                               const int* block_table_row, int max_blocks, int block_size, int n_blocks, int Hkv,
+                               int head_dim, void* kstage, void* vstage, cudaStream_t stream) {
+  const int shift = paged_block_shift(block_size);
+  MM_CHECK_ARG(shift >= 0, "mm_kv_dequant_paged: block_size must be a power of two in [16,256] (got %d)", block_size);
+  MM_CHECK_ARG(block_table_row != nullptr, "mm_kv_dequant_paged: block table missing");
+  MM_CHECK_ARG(kscale != nullptr && vscale != nullptr, "mm_kv_dequant_paged: scale arrays missing");
+  MM_CHECK_ARG(head_dim == DA_D && Hkv >= 1 && n_blocks >= 0 && n_blocks <= max_blocks,
+               "mm_kv_dequant_paged: need head_dim 128, Hkv >= 1 and 0 <= n_blocks <= max_blocks");
+  if (n_blocks == 0) return MM_OK;
+  const long long total = ((long long)n_blocks * Hkv * block_size) * (DA_D / 16) * 2;
+  long long blocks = ceil_div64(total, 256);
+  if (blocks > (long long)mm_num_sms() * 16) blocks = (long long)mm_num_sms() * 16;
+  kv_dequant_paged_kernel<<<(int)blocks, 256, 0, stream>>>((const uint8_t*)kpool, (const uint8_t*)vpool, kscale,
+                                                           vscale, block_table_row, n_blocks, Hkv, shift,
+                                                           (bf16*)kstage, (bf16*)vstage);
+  MM_CHECK_LAUNCH();
+  return MM_OK;
 }
 
 MM_API int mm_kv_prefill_paged(const void* qkv, long long ld, void* kpool, void* vpool, const int* block_table_row,

@@ -15,7 +15,7 @@ import torch
 from .. import ops
 from ..constants import EOS_TOKEN_IDS, IMAGE_END_TOKEN_ID, IMAGE_START_TOKEN_ID
 from .decode_step import decode_heads, decoder_stack_step
-from .llama import StackContext
+from .llama import FP8KVStore, StackContext
 from .logprobs import LogprobBuffers, check_logprobs
 from .sampling import SamplingArrays, SamplingParams, per_sequence
 
@@ -34,6 +34,27 @@ def check_forced_tokens(forced_tokens: Optional[torch.Tensor], embed_rows: int) 
                          f"embedding table's {embed_rows} rows (got min {lo}, max {hi})")
 
 
+KV_CACHE_DTYPES = ("bf16", "fp8_e4m3")
+
+
+def check_kv_cache_dtype(kv_cache_dtype) -> None:
+    """'bf16' (the default cache) or 'fp8_e4m3' (E4M3 rows with one power-of-two scale each, DESIGN.md §1). Raises
+    ValueError on the host, before any device work."""
+    if not isinstance(kv_cache_dtype, str) or kv_cache_dtype not in KV_CACHE_DTYPES:
+        raise ValueError(f"kv_cache_dtype must be one of {KV_CACHE_DTYPES} (got {kv_cache_dtype!r})")
+
+
+def alloc_kv_cache(kv_cache_dtype: str, shape, dev):
+    """(kc, vc, scales) for a cache of `shape` [..., dh]: bf16 and scales None, or uint8 E4M3 bytes and (ks, vs) fp32
+    [...] (one scale per row). Zero-filled."""
+    if kv_cache_dtype == "bf16":
+        kc = torch.zeros(shape, dtype=torch.bfloat16, device=dev)
+        return kc, torch.zeros_like(kc), None
+    kc = torch.zeros(shape, dtype=torch.uint8, device=dev)
+    ks = torch.zeros(shape[:-1], dtype=torch.float32, device=dev)
+    return kc, torch.zeros_like(kc), (ks, torch.zeros_like(ks))
+
+
 class DecodeEngine:
     def __init__(self, model):
         self.m = model
@@ -46,7 +67,7 @@ class DecodeEngine:
                  forced_tokens: Optional[torch.Tensor] = None, poll_every: int = 16,
                  max_steps: Optional[int] = None,
                  sampling: Union[None, SamplingParams, Sequence[SamplingParams]] = None,
-                 logprobs: Optional[int] = None):
+                 logprobs: Optional[int] = None, kv_cache_dtype: str = "bf16"):
         """inputs_embeds [B, P, H] (right-padded to P; prompt_lens[b] valid rows). B <= 128.
         sampling: None (greedy), one SamplingParams (sequence b draws with seed + b) or one per sequence. The draw
         replaces the argmax only: image mode, the EOS test on the drawn token and forced tokens are unchanged. When
@@ -58,9 +79,14 @@ class DecodeEngine:
         logprobs: None, or an int n in [0, 20]: every sequence also reports, for each id it emits, that id's
         log-probability under the step's raw distribution and the n most likely ids with theirs (engine/logprobs.py).
         Anything else raises ValueError before any device work. Ids and embeddings do not change.
+        kv_cache_dtype: 'bf16' (default) or 'fp8_e4m3': the KV cache holds E4M3 rows with one power-of-two scale each
+        (half the bytes), and every attention, prefill and decode, reads the values the cache holds. Right-padded
+        prompts quantise their pad rows like any other row; nothing reads them. Anything else raises ValueError before
+        any device work.
         Returns (ids list per sequence (int32 tensors), image_embeds list per sequence [n, C]), and with logprobs a
         third element: one TokenLogprobs per sequence, entry k belonging to ids[k]."""
         check_logprobs(logprobs)
+        check_kv_cache_dtype(kv_cache_dtype)
         B, P, H = inputs_embeds.shape
         assert B <= 128, f"decode batch is limited to 128 sequences per step (got {B}): the weight-streaming GEMM " \
                          "serves at most 128 batch rows"
@@ -90,8 +116,7 @@ class DecodeEngine:
         eos0 = eos[0] if eos else -1
         eos1 = eos[1] if len(eos) > 1 else eos0
 
-        kc = torch.zeros((L, B, Hkv, Tmax, dh), dtype=torch.bfloat16, device=dev)
-        vc = torch.zeros_like(kc)
+        kc, vc, scales = alloc_kv_cache(kv_cache_dtype, (L, B, Hkv, Tmax, dh), dev)
 
         # ---- prefill: full-sequence kernels, K/V captured into the cache
         pos = torch.arange(P, dtype=torch.int32).repeat(B).to(dev)
@@ -99,6 +124,11 @@ class DecodeEngine:
         layers = [l.weights() for l in model.layers]
         x = inputs_embeds.reshape(B * P, H).contiguous()
         for i, w in enumerate(layers):
+            if scales is not None:
+                x = stack.layer_forward(w, x, ctx, save=True, save_gu=False,
+                                        kv=FP8KVStore(kc[i], vc[i], scales[0][i], scales[1][i]))
+                ctx.saved.pop()
+                continue
             x = stack.layer_forward(w, x, ctx, save=True, save_gu=False)
             s = ctx.saved.pop()
             ops.kv_prefill(s.qkv, kc[i], vc[i], B, P, Hq, Hkv, dh)
@@ -140,7 +170,7 @@ class DecodeEngine:
 
         def one_step_body():
             # position of the token being fed = pos - 1 (the state step already advanced pos)
-            return decoder_stack_step(layers, xin, kc, vc, st["pos"] - 1, stack)
+            return decoder_stack_step(layers, xin, kc, vc, st["pos"] - 1, stack, scales=scales)
 
         # One captured CUDA graph is replayed for every step (launch-bound inner loop): all per-step state,
         # including the index into the forced-token schedule, lives in device memory.

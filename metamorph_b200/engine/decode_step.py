@@ -9,16 +9,24 @@ import torch
 from .. import ops
 
 
-def decoder_stack_step(layers, x, kc, vc, cur_pos, stack, table=None):
+def decoder_stack_step(layers, x, kc, vc, cur_pos, stack, table=None, scales=None):
     """x [B, H] -> [B, H] through all layers; K/V of the fed position are appended to kc/vc [L, B, Hkv, Tmax, dh].
     With a block table [B, max_blocks] (int32, device) kc/vc are paged pools [L, num_blocks, Hkv, block_size, dh] and
-    the attention addresses them through it (ops.decode_attn_paged: the same bits as the dense cache)."""
+    the attention addresses them through it (ops.decode_attn_paged: the same bits as the dense cache).
+    scales: None (bf16 cache), or the (ks, vs) fp32 scale arrays of an FP8 cache ([L, B, Hkv, Tmax] dense, [L,
+    num_blocks, Hkv, block_size] paged; kc/vc are then uint8 E4M3 bytes) for the FP8 attention kernels."""
     d = stack.dims
     Hq, Hkv, dh = d.n_heads, d.n_kv_heads, d.head_dim
     for i, w in enumerate(layers):
         n1 = ops.rmsnorm(x, w.ln1, d.rms_eps)
         qkv = ops.skinny_gemm(n1, w.wqkv)
-        if table is None:
+        if scales is not None and table is None:
+            attn = ops.decode_attn_fp8(qkv, kc[i], vc[i], scales[0][i], scales[1][i], cur_pos, stack.cos, stack.sin,
+                                       Hq, Hkv, dh, stack.scale)
+        elif scales is not None:
+            attn = ops.decode_attn_paged_fp8(qkv, kc[i], vc[i], scales[0][i], scales[1][i], table, cur_pos, stack.cos,
+                                             stack.sin, Hq, Hkv, dh, stack.scale)
+        elif table is None:
             attn = ops.decode_attn(qkv, kc[i], vc[i], cur_pos, stack.cos, stack.sin, Hq, Hkv, dh, stack.scale)
         else:
             attn = ops.decode_attn_paged(qkv, kc[i], vc[i], table, cur_pos, stack.cos, stack.sin, Hq, Hkv, dh,

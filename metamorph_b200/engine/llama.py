@@ -121,6 +121,41 @@ class PagedPrefill:
     q_start: int
 
 
+@dataclass
+class FP8KVStore:
+    """One layer's FP8 KV cache (E4M3 bytes + one fp32 scale per (position, kv head) row, ops.kv_quant_prefill) for the
+    rows of a prefill. `layer_forward` quantises their post-RoPE K/V into it right after RoPE and attends over what it
+    holds: the K/V columns of qkv are overwritten with the dequantised rows.
+      dense (table_row None): kc / vc [B, Hkv, Tmax, dh] uint8, ks / vs [B, Hkv, Tmax] fp32, rows = B sequences of T;
+      paged: pools [num_blocks, Hkv, block_size, dh] and scales [num_blocks, Hkv, block_size]; the rows are positions
+        q_start .. q_start + T - 1 of ONE sequence, written through its table row. With q_start > 0 (a cached prefix of
+        q_start positions, a block multiple) `staging` = (kst, vst, identity row) holds bf16 pools [max_blocks, Hkv,
+        block_size, dh]: the prefix blocks are dequantised into them, the new rows follow, and attention reads keys
+        0 .. q_start + T - 1 from there (ops.attn_fwd_paged), so it sees exactly the values the cache holds."""
+    kc: torch.Tensor
+    vc: torch.Tensor
+    ks: torch.Tensor
+    vs: torch.Tensor
+    table_row: Optional[torch.Tensor] = None
+    q_start: int = 0
+    staging: Optional[tuple] = None
+
+    def write(self, qkv: torch.Tensor, B: int, T: int, Hq: int, Hkv: int, dh: int) -> None:
+        if self.table_row is None:
+            ops.kv_quant_prefill(qkv, self.kc, self.vc, self.ks, self.vs, B, T, Hq, Hkv, dh)
+            return
+        bs = self.kc.shape[2]
+        assert B == 1 and self.q_start % bs == 0 and (self.q_start == 0 or self.staging is not None), \
+            "a paged FP8 prefill continues one sequence at a block boundary, through staging after a prefix"
+        first = self.q_start // bs
+        if self.staging is not None:
+            kst, vst, ident = self.staging
+            ops.kv_dequant_paged(self.kc, self.vc, self.ks, self.vs, self.table_row, first, kst, vst)
+        ops.kv_quant_prefill_paged(qkv, self.kc, self.vc, self.ks, self.vs, self.table_row[first:], T, Hq, Hkv, dh)
+        if self.staging is not None:
+            ops.kv_prefill_paged(qkv, kst, vst, ident[first:], T, Hq, Hkv, dh)
+
+
 class LlamaStack:
     """Forward/backward over a list of LayerWeights. Stateless apart from the RoPE tables."""
 
@@ -137,9 +172,12 @@ class LlamaStack:
 
     # ------------------------------------------------------------------ forward
     def layer_forward(self, w: LayerWeights, x: torch.Tensor, ctx: StackContext, save: bool,
-                      save_gu: bool, paged: Optional[PagedPrefill] = None) -> torch.Tensor:
+                      save_gu: bool, paged: Optional[PagedPrefill] = None,
+                      kv: Optional[FP8KVStore] = None) -> torch.Tensor:
         """paged: the rows continue a sequence cached in a paged pool (prefix caching). Their post-RoPE K/V are written
-        into the pool blocks from position q_start on, and attention reads keys 0 .. q_start + T - 1 from the pool."""
+        into the pool blocks from position q_start on, and attention reads keys 0 .. q_start + T - 1 from the pool.
+        kv: an FP8 cache the rows' post-RoPE K/V are quantised into before attention, which then reads the dequantised
+        values (FP8KVStore); None keeps the bf16 path."""
         d = self.dims
         B, T = ctx.B, ctx.T
         Hq, Hkv, dh = d.n_heads, d.n_kv_heads, d.head_dim
@@ -148,7 +186,12 @@ class LlamaStack:
         del n1
         ops.rope_(qkv, ctx.pos, self.cos, self.sin, Hq + Hkv, dh)
         q, k, v = qkv[:, :Hq * dh], qkv[:, Hq * dh:(Hq + Hkv) * dh], qkv[:, (Hq + Hkv) * dh:]
-        if paged is not None:
+        if kv is not None:
+            kv.write(qkv, B, T, Hq, Hkv, dh)
+        if kv is not None and kv.staging is not None:
+            kst, vst, ident = kv.staging
+            attn, lse = ops.attn_fwd_paged(q, kst, vst, ident, kv.q_start, Hq, Hkv, dh, self.scale), None
+        elif paged is not None:
             bs = paged.kpool.shape[2]
             assert B == 1 and paged.q_start % bs == 0, "a paged prefill continues one sequence at a block boundary"
             ops.kv_prefill_paged(qkv, paged.kpool, paged.vpool, paged.table_row[paged.q_start // bs:], x.shape[0], Hq,

@@ -23,6 +23,11 @@ A paged server also caches prompt prefixes: `h = cache_prefix(prefix)` prefills 
 `submit(suffix, prefix=h)` shares them and prefills only the prefix tail and the suffix (attention reads the shared
 keys through the block table, `ops.attn_fwd_paged`), and `drop_prefix(h)` lets the blocks go once no request uses them.
 The request returns the bits of the whole prompt submitted without a prefix.
+With `kv_cache_dtype="fp8_e4m3"` the cache (dense or paged) holds E4M3 rows with one power-of-two scale each, half the
+bytes of bf16: every prefill quantises its K/V into the cache before its attention and attends over the dequantised
+values, and the decode step runs the FP8 attention kernels. A prefixed prefill dequantises the shared blocks into a
+per-server bf16 staging pool and attends there. A row's bytes depend on that row alone, so paged equals dense, a prefixed
+request equals its whole prompt and a request does not depend on its neighbours, exactly as on a bf16 server.
 A request may ask for token log-probabilities (`submit(..., logprobs=n)`): while one is in flight the step runs a graph
 that adds the logprob kernel after the state step (captured the first time it is needed, for the greedy and the sampled
 step alike); its slot's `n_top` is written on admission, -1 for every request that did not ask. The kernel only reads
@@ -40,9 +45,9 @@ import torch
 
 from .. import ops
 from ..constants import EOS_TOKEN_IDS, IMAGE_END_TOKEN_ID, IMAGE_START_TOKEN_ID
-from .decode import check_forced_tokens
+from .decode import alloc_kv_cache, check_forced_tokens, check_kv_cache_dtype
 from .decode_step import decode_heads, decoder_stack_step
-from .llama import PagedPrefill, StackContext
+from .llama import FP8KVStore, PagedPrefill, StackContext
 from .logprobs import LogprobBuffers, TokenLogprobs, cat as cat_logprobs, check_logprobs
 from .sampling import SamplingArrays, SamplingParams
 
@@ -160,11 +165,15 @@ class ContinuousBatcher:
     def __init__(self, model, max_slots: int = 8, max_context: int = 2048, max_new_tokens: int = 1024,
                  poll_every: int = 8, use_cuda_graph: bool = True, start_image_token_id: int = IMAGE_START_TOKEN_ID,
                  end_image_token_id: int = IMAGE_END_TOKEN_ID, eos_token_id=EOS_TOKEN_IDS,
-                 kv_pool_tokens: Optional[int] = None, kv_block_size: int = 64):
+                 kv_pool_tokens: Optional[int] = None, kv_block_size: int = 64, kv_cache_dtype: str = "bf16"):
         """kv_pool_tokens: None keeps one dense cache region of max_context positions per slot. An integer gives a
         paged cache: a pool of ceil(kv_pool_tokens / kv_block_size) blocks (plus one scratch block) shared by all
         slots; a request is admitted (strictly first come, first served) once a slot and the blocks it needs
-        are free. max_context stays the longest request either way."""
+        are free. max_context stays the longest request either way.
+        kv_cache_dtype: 'bf16' or 'fp8_e4m3' (E4M3 rows + one fp32 scale per row: 1 byte per element plus 4 per row, so
+        a pool of the same bytes holds about 1.94x the positions; kv_pool_tokens still counts positions). Anything else
+        raises ValueError before any device work."""
+        check_kv_cache_dtype(kv_cache_dtype)
         assert 1 <= max_slots <= 128, f"the weight-streaming step serves at most 128 sequences (max_slots={max_slots})"
         check_kv_block_size(kv_block_size)
         if kv_pool_tokens is not None and (not isinstance(kv_pool_tokens, int) or kv_pool_tokens < 1):
@@ -189,17 +198,26 @@ class ContinuousBatcher:
         self.eos1 = eos[1] if len(eos) > 1 else self.eos0
         self.start_id, self.end_id = start_image_token_id, end_image_token_id
         self.stack.ensure_positions(max_context + 1)
+        self.kv_cache_dtype = kv_cache_dtype
+        self.staging = None
         if kv_pool_tokens is None:
             self.alloc, self.table = None, None
-            self.kc = torch.zeros((self.L, B, d.n_kv_heads, max_context, d.head_dim), dtype=torch.bfloat16, device=dev)
+            self.kc, self.vc, self.scales = alloc_kv_cache(
+                kv_cache_dtype, (self.L, B, d.n_kv_heads, max_context, d.head_dim), dev)
         else:
             self.alloc = KVBlockAllocator(-(-kv_pool_tokens // kv_block_size), kv_block_size)
             self.max_blocks = -(-max_context // kv_block_size)
-            # pools [L, num_blocks + scratch, Hkv, block_size, dh]; table rows start (and return to) all scratch
-            self.kc = torch.zeros((self.L, self.alloc.num_blocks + 1, d.n_kv_heads, kv_block_size, d.head_dim),
-                                  dtype=torch.bfloat16, device=dev)
+            # pools [L, num_blocks + scratch, Hkv, block_size, dh]; table rows start (and return to) all scratch. The
+            # scratch block's FP8 scale rows, like its data, are written only by frozen slots.
+            self.kc, self.vc, self.scales = alloc_kv_cache(
+                kv_cache_dtype, (self.L, self.alloc.num_blocks + 1, d.n_kv_heads, kv_block_size, d.head_dim), dev)
             self.table = torch.full((B, self.max_blocks), self.alloc.scratch, dtype=torch.int32, device=dev)
-        self.vc = torch.zeros_like(self.kc)
+            if self.scales is not None:
+                # bf16 staging for prefixed FP8 prefills: one sequence's blocks at their table index, reused by every
+                # layer and admission
+                kst = torch.zeros((self.max_blocks, d.n_kv_heads, kv_block_size, d.head_dim), dtype=torch.bfloat16,
+                                  device=dev)
+                self.staging = (kst, torch.zeros_like(kst), torch.arange(self.max_blocks, dtype=torch.int32, device=dev))
         self.st = {k: torch.zeros(B, dtype=torch.int32, device=dev) for k in
                    ("in_image_mode", "total_image_tokens", "total_output", "n_ids", "n_img", "append_kind",
                     "next_token")}
@@ -234,7 +252,8 @@ class ContinuousBatcher:
     # ------------------------------------------------------------------ one device step for all slots
     def _step_body(self, sampled: bool = False, logprobs: bool = False):
         st = self.st
-        x = decoder_stack_step(self.layers, self.xin, self.kc, self.vc, st["pos"] - 1, self.stack, self.table)
+        x = decoder_stack_step(self.layers, self.xin, self.kc, self.vc, st["pos"] - 1, self.stack, self.table,
+                               self.scales)
         tok, pred_z, prediction = decode_heads(self.m, x, st["in_image_mode"], self.logits, self.V,
                                                self.samp if sampled else None, st["total_output"])
         ops.decode_state_step_slots(st, tok, self.forced, self.max_new_slot, self.B, self.ntok, self.start_id,
@@ -377,6 +396,12 @@ class ContinuousBatcher:
         ctx = StackContext(B=1, T=Ls, pos=torch.arange(Ls, dtype=torch.int32, device=self.dev), seqlens=None)
         x = e[:Ls]
         for i, w in enumerate(self.layers):
+            if self.scales is not None:
+                x = self.stack.layer_forward(w, x, ctx, save=True, save_gu=False,
+                                             kv=FP8KVStore(self.kc[i], self.vc[i], self.scales[0][i],
+                                                           self.scales[1][i], row))
+                ctx.saved.pop()
+                continue
             x = self.stack.layer_forward(w, x, ctx, save=True, save_gu=False)
             s = ctx.saved.pop()
             ops.kv_prefill_paged(s.qkv, self.kc[i], self.vc[i], row, Ls, Hq, Hkv, dh)
@@ -413,6 +438,11 @@ class ContinuousBatcher:
                 ctx = StackContext(B=1, T=P - 1, pos=pos, seqlens=None)
                 x = req.embeds[:P - 1].contiguous()
                 for i, w in enumerate(self.layers):
+                    if self.scales is not None:
+                        x = self.stack.layer_forward(w, x, ctx, save=False, save_gu=False,
+                                                     kv=FP8KVStore(self.kc[i], self.vc[i], self.scales[0][i],
+                                                                   self.scales[1][i], self.table[b], Ls, self.staging))
+                        continue
                     x = self.stack.layer_forward(w, x, ctx, save=False, save_gu=False,
                                                  paged=PagedPrefill(self.kc[i], self.vc[i], self.table[b], Ls))
             P += Ls
@@ -421,6 +451,13 @@ class ContinuousBatcher:
             ctx = StackContext(B=1, T=P - 1, pos=pos, seqlens=None)
             x = req.embeds[:P - 1].contiguous()
             for i, w in enumerate(self.layers):
+                if self.scales is not None:
+                    ks, vs = self.scales[0][i], self.scales[1][i]
+                    kv = FP8KVStore(self.kc[i, b:b + 1], self.vc[i, b:b + 1], ks[b:b + 1], vs[b:b + 1]) \
+                        if self.alloc is None else FP8KVStore(self.kc[i], self.vc[i], ks, vs, self.table[b])
+                    x = self.stack.layer_forward(w, x, ctx, save=True, save_gu=False, kv=kv)
+                    ctx.saved.pop()
+                    continue
                 x = self.stack.layer_forward(w, x, ctx, save=True, save_gu=False)
                 s = ctx.saved.pop()
                 if self.alloc is None:

@@ -534,6 +534,79 @@ def kv_prefill_paged(qkv, kpool, vpool, table_row, T, Hq, Hkv, head_dim):
          stream_ptr())
 
 
+def decode_attn_fp8(qkv, kcache, vcache, kscale, vscale, pos, cos, sin, Hq, Hkv, head_dim, scale, out=None,
+                    splits=None):
+    """decode_attn on an FP8 cache: kcache / vcache [B, Hkv, Tmax, head_dim] uint8 (E4M3 bytes), kscale / vscale
+    [B, Hkv, Tmax] fp32 (one power-of-two scale per row). With equal `splits` the output bits are decode_attn's on a bf16
+    cache holding the dequantised rows; the new k / v are quantised and appended (include/metamorph_b200.h)."""
+    require_cuda(qkv, kcache, vcache, kscale, vscale, pos, cos, sin)
+    assert kcache.dtype == torch.uint8 and vcache.dtype == torch.uint8, "FP8 caches hold uint8 E4M3 bytes"
+    assert kscale.dtype == torch.float32 and kscale.shape == kcache.shape[:3] and vscale.shape == kscale.shape
+    B = qkv.shape[0]
+    Tmax = kcache.shape[2]
+    if splits is None:
+        splits = _decode_attn_splits(B, Hkv, qkv.device)
+    if out is None:
+        out = torch.empty((B, Hq * head_dim), dtype=torch.bfloat16, device=qkv.device)
+    ws = _workspace("decode_attn", B * Hkv * splits * (Hq // Hkv) * (2 + head_dim) * 4, qkv.device)
+    call("mm_decode_attn_fp8", ptr(qkv), ll(qkv.stride(0)), ptr(kcache), ptr(vcache), ptr(kscale), ptr(vscale),
+         ptr(pos), ptr(cos), ptr(sin), ptr(out), ll(out.stride(0)), c_int(B), c_int(Hq), c_int(Hkv), c_int(head_dim),
+         c_int(Tmax), c_float(scale), ptr(ws), ll(ws.numel()), c_int(splits), stream_ptr())
+    return out
+
+
+def decode_attn_paged_fp8(qkv, kpool, vpool, kscale, vscale, table, pos, cos, sin, Hq, Hkv, head_dim, scale, out=None,
+                          splits=None):
+    """decode_attn_paged on FP8 pools: kpool / vpool [num_blocks, Hkv, block_size, head_dim] uint8, kscale / vscale
+    [num_blocks, Hkv, block_size] fp32. With equal `splits`, the bits of decode_attn_fp8 on the same logical cache."""
+    require_cuda(qkv, kpool, vpool, kscale, vscale, table, pos, cos, sin)
+    assert kpool.dtype == torch.uint8 and vpool.dtype == torch.uint8, "FP8 pools hold uint8 E4M3 bytes"
+    assert kscale.dtype == torch.float32 and kscale.shape == kpool.shape[:3] and vscale.shape == kscale.shape
+    assert table.dtype == torch.int32 and table.dim() == 2 and table.is_contiguous(), "table: [B, max_blocks] int32"
+    B = qkv.shape[0]
+    assert table.shape[0] >= B
+    if splits is None:
+        splits = _decode_attn_splits(B, Hkv, qkv.device)
+    if out is None:
+        out = torch.empty((B, Hq * head_dim), dtype=torch.bfloat16, device=qkv.device)
+    ws = _workspace("decode_attn", B * Hkv * splits * (Hq // Hkv) * (2 + head_dim) * 4, qkv.device)
+    call("mm_decode_attn_paged_fp8", ptr(qkv), ll(qkv.stride(0)), ptr(kpool), ptr(vpool), ptr(kscale), ptr(vscale),
+         ptr(table), c_int(table.shape[1]), c_int(kpool.shape[2]), ptr(pos), ptr(cos), ptr(sin), ptr(out),
+         ll(out.stride(0)), c_int(B), c_int(Hq), c_int(Hkv), c_int(head_dim), c_float(scale), ptr(ws), ll(ws.numel()),
+         c_int(splits), stream_ptr())
+    return out
+
+
+def kv_quant_prefill(qkv, kcache, vcache, kscale, vscale, B, T, Hq, Hkv, head_dim):
+    """kv_prefill into an FP8 cache ([B', Hkv, Tmax, head_dim] uint8 + [B', Hkv, Tmax] fp32 scales, B <= B'); the K / V
+    columns of qkv [B*T, *] become the dequantised rows the cache holds."""
+    require_cuda(qkv, kcache, vcache, kscale, vscale)
+    assert kcache.dtype == torch.uint8 and kscale.dtype == torch.float32 and kscale.shape == kcache.shape[:3]
+    call("mm_kv_quant_prefill", ptr(qkv), ll(qkv.stride(0)), ptr(kcache), ptr(vcache), ptr(kscale), ptr(vscale),
+         c_int(B), c_int(T), c_int(Hq), c_int(Hkv), c_int(head_dim), c_int(kcache.shape[2]), stream_ptr())
+
+
+def kv_quant_prefill_paged(qkv, kpool, vpool, kscale, vscale, table_row, T, Hq, Hkv, head_dim):
+    """kv_quant_prefill for one sequence into the blocks of its table row (table_row [max_blocks] int32, device)."""
+    require_cuda(qkv, kpool, vpool, kscale, vscale, table_row)
+    assert kpool.dtype == torch.uint8 and kscale.dtype == torch.float32 and kscale.shape == kpool.shape[:3]
+    assert table_row.dtype == torch.int32 and table_row.dim() == 1 and table_row.stride(0) == 1
+    call("mm_kv_quant_prefill_paged", ptr(qkv), ll(qkv.stride(0)), ptr(kpool), ptr(vpool), ptr(kscale), ptr(vscale),
+         ptr(table_row), c_int(table_row.shape[0]), c_int(kpool.shape[2]), c_int(T), c_int(Hq), c_int(Hkv),
+         c_int(head_dim), stream_ptr())
+
+
+def kv_dequant_paged(kpool, vpool, kscale, vscale, table_row, n_blocks, kstage, vstage):
+    """Staging block i of the bf16 pools kstage / vstage <- the dequantised pool block table_row[i], i < n_blocks."""
+    require_cuda(kpool, vpool, kscale, vscale, table_row, kstage, vstage)
+    assert kpool.dtype == torch.uint8 and kstage.dtype == torch.bfloat16 and kstage.shape[1:] == kpool.shape[1:]
+    assert kstage.shape[0] >= n_blocks and vstage.shape == kstage.shape and kstage.is_contiguous()
+    assert table_row.dtype == torch.int32 and table_row.dim() == 1 and table_row.stride(0) == 1
+    call("mm_kv_dequant_paged", ptr(kpool), ptr(vpool), ptr(kscale), ptr(vscale), ptr(table_row),
+         c_int(table_row.shape[0]), c_int(kpool.shape[2]), c_int(n_blocks), c_int(kpool.shape[1]),
+         c_int(kpool.shape[3]), ptr(kstage), ptr(vstage), stream_ptr())
+
+
 def attn_fwd_paged(q, kpool, vpool, table_row, q_start, Hq, Hkv, head_dim, scale, out=None):
     """Causal attention of the query rows of positions q_start .. q_start + n_q - 1 (q: [n_q, *] row-major view, e.g. the
     Q columns of a fused qkv) over keys / values 0 .. q_start + n_q - 1 of a paged pool (kpool / vpool [num_blocks, Hkv,
