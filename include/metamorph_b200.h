@@ -259,6 +259,27 @@ int mm_kv_quant_prefill_paged(void* qkv, long long ld, void* kpool, void* vpool,
 int mm_kv_dequant_paged(const void* kpool, const void* vpool, const float* kscale, const float* vscale,
                         const int* block_table_row, int max_blocks, int block_size, int n_blocks, int Hkv,
                         int head_dim, void* kstage, void* vstage, cudaStream_t s);
+/* FP8 weights (E4M3) for the weight-streaming GEMMs. A matrix W [N, K] (K a multiple of 128) is stored as bytes
+ * q [N, K] (row stride ldq / ldw, in bytes) and fp32 scales [N, K / 128] (row stride lds): group j of row n,
+ * W[n, 128 j .. 128 j + 127], is one row of the FP8 KV-cache rule above, so W-hat = float(q) * scale is exact and a bf16
+ * value.
+ * mm_weight_quant_fp8: W (bf16, row stride ldw elements) -> (q, scale); mm_weight_dequant_fp8: (q, scale) -> W-hat (bf16,
+ * row stride ldw elements). One warp per group; row strides must be multiples of 4 and at least K.
+ * mm_skinny_gemm_fp8 / mm_skinny_gemm_wide_fp8: mm_skinny_gemm / mm_skinny_gemm_wide with W given as (Wq, wscale), same
+ * batch limits, epilogues and out_f32 / padded ldy. Every weight reaches the tensor cores as its exact bf16 value W-hat,
+ * in the bf16 kernel's fragment slots and accumulation order (the same k chunks per warp, the same split-K and reduction),
+ * so the output bits are those of the bf16 call on W-hat. Need K % 128 == 0, ldw % 16 == 0, lds >= K / 128, 16-byte
+ * aligned x / Wq and a non-null, 4-byte aligned wscale; checked before any launch. */
+int mm_weight_quant_fp8(const void* W, long long ldw, void* q, long long ldq, float* scale, long long lds, int N, int K,
+                        cudaStream_t s);
+int mm_weight_dequant_fp8(const void* q, long long ldq, const float* scale, long long lds, void* W, long long ldw, int N,
+                          int K, cudaStream_t s);
+int mm_skinny_gemm_fp8(const void* x, const void* Wq, const float* wscale, void* y, const void* bias, const void* resid,
+                       long long ldx, long long ldw, long long lds, long long ldy, long long ldr, int m, int N, int K,
+                       int epilogue, int out_f32, cudaStream_t s);
+int mm_skinny_gemm_wide_fp8(const void* x, const void* Wq, const float* wscale, void* y, const void* bias,
+                            const void* resid, long long ldx, long long ldw, long long lds, long long ldy, long long ldr,
+                            int m, int N, int K, int epilogue, int out_f32, cudaStream_t s);
 int mm_decode_state_step(int* in_image_mode, int* total_image_tokens, int* total_output, int* finished, int* pos,
                          int* n_ids, int* n_img, int* ids_out, int* append_kind, int* next_token,
                          const int* argmax_tok, const int* forced, int forced_ld, int step, int B,

@@ -13,7 +13,7 @@
 //   decode_state  the per-sequence text/image mode state machine of greedy_decode
 //                 (metamorph_llama.py:547-582) on the device: no .item() host syncs.
 #include "common.cuh"
-#include <cuda_fp8.h>
+#include "fp8.cuh"
 #include <mutex>
 #include <type_traits>
 #include <stdlib.h>
@@ -37,17 +37,23 @@ constexpr int SK2_STAGES = 8;      // default ring depth (16-row slabs: 8 x 8 KB
 constexpr int SK2_KT = 256;      // k elements per stage
 constexpr int SK2_THREADS = 160; // warp 0 = TMA producer, warps 1..4 = consumers
 
-template <int ROWS, int NST = SK2_STAGES, int NB = 1>
-__global__ void __launch_bounds__(SK2_THREADS)
-skinny_gemm_tma_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
-                       void* __restrict__ y, long long ldy, const bf16* __restrict__ bias,
-                       const bf16* __restrict__ resid, long long ldr, int m, int N, int K, int epi, int out_f32) {
+// FP8 (skinny_gemm_fp8_kernel): the weight slab is E4M3 bytes with one power-of-two fp32 scale per 128 k of a row
+// (fp8_quant_row_warp); a stage holds 2 uint8 boxes [ROWS x 128 k] (one 128-byte swizzled row = 128 k) instead of 4 bf16
+// boxes [ROWS x 64 k]. Each lane loads the 8 bytes of exactly the 8 k its bf16 counterpart loads, turns them into
+// float(q) * scale (exact, a bf16 value) in the same four bf16x2 registers, and the same mma.sync sequence follows: on
+// weights W-hat = float(q) * scale the output bits are skinny_gemm_tma_kernel's.
+template <int ROWS, int NST, int NB, bool FP8>
+__device__ __forceinline__ void
+skinny_gemm_body(const CUtensorMap& tmap_w, const CUtensorMap& tmap_x, void* __restrict__ y, long long ldy,
+                 const bf16* __restrict__ bias, const bf16* __restrict__ resid, long long ldr, int m, int N, int K, int epi,
+                 int out_f32, const float* __restrict__ wsc, long long lds) {
   constexpr int G = ROWS >= 16 ? ROWS / 16 : 1;
   constexpr bool HALF = ROWS == 8;             // 8-row slab: rows 8..15 of the MMA operand are zero
   constexpr int MB = 8 * NB;                   // batch rows served: NB n8 tiles of the MMA's B operand
-  constexpr int BOX = ROWS * 128;              // bytes of one [ROWS x 64 k] weight box
+  constexpr int BOX = ROWS * 128;              // bytes of one weight box: [ROWS x 64 k] bf16 or [ROWS x 128 k] E4M3
+  constexpr int NBOX = FP8 ? 2 : 4;            // weight boxes per stage of 256 k
   constexpr int XBOX = MB * 128;               // bytes of one [MB batch rows x 64 k] activation box
-  constexpr int STAGE_W = 4 * BOX;             // 4 boxes = 256 k of the weight slab
+  constexpr int STAGE_W = NBOX * BOX;          // 256 k of the weight slab
   constexpr int STAGE = STAGE_W + 4 * XBOX;    // + the same 256 k of the activations (rows >= m zero-filled by TMA)
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -80,8 +86,8 @@ skinny_gemm_tma_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
       for (int kt = 0; kt < n_pre; ++kt) {
         mbar_arrive_expect_tx(bar + 8 * kt, STAGE);
 #pragma unroll
-        for (int bx = 0; bx < 4; ++bx)
-          tma_load_2d(base + kt * STAGE + bx * BOX, &tmap_w, bar + 8 * kt, kt * SK2_KT + bx * 64, n0);
+        for (int bx = 0; bx < NBOX; ++bx)
+          tma_load_2d(base + kt * STAGE + bx * BOX, &tmap_w, bar + 8 * kt, kt * SK2_KT + bx * (FP8 ? 128 : 64), n0);
       }
       griddep_wait();
       for (int kt = 0; kt < n_pre; ++kt) {
@@ -95,8 +101,8 @@ skinny_gemm_tma_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
         mbar_wait(bar + 8 * (NST + s), ph ^ 1);
         mbar_arrive_expect_tx(bar + 8 * s, STAGE);
 #pragma unroll
-        for (int bx = 0; bx < 4; ++bx)
-          tma_load_2d(base + s * STAGE + bx * BOX, &tmap_w, bar + 8 * s, kt * SK2_KT + bx * 64, n0);
+        for (int bx = 0; bx < NBOX; ++bx)
+          tma_load_2d(base + s * STAGE + bx * BOX, &tmap_w, bar + 8 * s, kt * SK2_KT + bx * (FP8 ? 128 : 64), n0);
 #pragma unroll
         for (int bx = 0; bx < 4; ++bx)
           tma_load_2d(base + s * STAGE + STAGE_W + bx * XBOX, &tmap_x, bar + 8 * s, kt * SK2_KT + bx * 64, 0);
@@ -115,6 +121,19 @@ skinny_gemm_tma_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
     for (int kt = 0; kt < n_kt; ++kt) {
       const int s = kt % NST;
       const uint32_t ph = (uint32_t)((kt / NST) & 1);
+      // FP8: the scales of this warp's 64 k (group 2 kt + cw / 2) for its rows r0 / r1 of every 16-row group, requested
+      // before the stage wait; rows past N and the group past K (zero-filled bytes) take 1
+      float sc0[G], sc1[G];
+      if constexpr (FP8) {
+        const int grp = 2 * kt + (cw >> 1);
+#pragma unroll
+        for (int i = 0; i < G; ++i) {
+          const int n = n0 + i * 16 + g;
+          const bool gok = grp * 128 < K;
+          sc0[i] = gok && n < N ? __ldg(wsc + (long long)n * lds + grp) : 1.f;
+          sc1[i] = gok && !HALF && n + 8 < N ? __ldg(wsc + (long long)(n + 8) * lds + grp) : 1.f;
+        }
+      }
       mbar_wait(bar + 8 * s, ph);
       const uint8_t* st = base_ptr + s * STAGE;
 #pragma unroll
@@ -122,6 +141,9 @@ skinny_gemm_tma_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
         const int cc = 2 * cw + u;             // k32 chunk of this stage: box cc/2, half cc%2
         const uint8_t* bx = st + (cc >> 1) * BOX;
         const int chunk = (cc & 1) * 4 + t;    // 16-byte chunk index inside the 128-byte row
+        // FP8: the same 8 k sit at byte 64 (cw & 1) + 8 chunk of a row of box cw / 2
+        const uint8_t* bx8 = st + (cw >> 1) * BOX;
+        const int c8 = 4 * (cw & 1) + (chunk >> 1), h8 = (chunk & 1) * 8;
         // B fragments: batch rows g + 8 nb, the same 8 k values (128-byte swizzled [MB x 64] box; the swizzle repeats
         // every 8 rows, so row g + 8 nb uses the same chunk permutation as row g)
         int4 xb[NB];
@@ -131,9 +153,23 @@ skinny_gemm_tma_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
 #pragma unroll
         for (int i = 0; i < G; ++i) {
           const int r0 = i * 16 + g, r1 = r0 + 8;
-          const int4 w0 = *reinterpret_cast<const int4*>(bx + r0 * 128 + ((chunk ^ (r0 & 7)) << 4));
-          const int4 w1 = HALF ? make_int4(0, 0, 0, 0)
-                               : *reinterpret_cast<const int4*>(bx + r1 * 128 + ((chunk ^ (r1 & 7)) << 4));
+          int4 w0, w1;
+          if constexpr (FP8) {
+            const uint2 q0 = *reinterpret_cast<const uint2*>(bx8 + r0 * 128 + ((c8 ^ (r0 & 7)) << 4) + h8);
+            const uint2 a0 = fp8x4_to_bf16x4(q0.x, sc0[i]), b0 = fp8x4_to_bf16x4(q0.y, sc0[i]);
+            w0 = make_int4((int)a0.x, (int)a0.y, (int)b0.x, (int)b0.y);
+            if (HALF) {
+              w1 = make_int4(0, 0, 0, 0);
+            } else {
+              const uint2 q1 = *reinterpret_cast<const uint2*>(bx8 + r1 * 128 + ((c8 ^ (r1 & 7)) << 4) + h8);
+              const uint2 a1 = fp8x4_to_bf16x4(q1.x, sc1[i]), b1 = fp8x4_to_bf16x4(q1.y, sc1[i]);
+              w1 = make_int4((int)a1.x, (int)a1.y, (int)b1.x, (int)b1.y);
+            }
+          } else {
+            w0 = *reinterpret_cast<const int4*>(bx + r0 * 128 + ((chunk ^ (r0 & 7)) << 4));
+            w1 = HALF ? make_int4(0, 0, 0, 0)
+                      : *reinterpret_cast<const int4*>(bx + r1 * 128 + ((chunk ^ (r1 & 7)) << 4));
+          }
           const uint32_t a1[4] = {(uint32_t)w0.x, (uint32_t)w1.x, (uint32_t)w0.y, (uint32_t)w1.y};
           const uint32_t a2[4] = {(uint32_t)w0.z, (uint32_t)w1.z, (uint32_t)w0.w, (uint32_t)w1.w};
 #pragma unroll
@@ -195,6 +231,55 @@ skinny_gemm_tma_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
   }
 }
 
+template <int ROWS, int NST = SK2_STAGES, int NB = 1>
+__global__ void __launch_bounds__(SK2_THREADS)
+skinny_gemm_tma_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
+                       void* __restrict__ y, long long ldy, const bf16* __restrict__ bias,
+                       const bf16* __restrict__ resid, long long ldr, int m, int N, int K, int epi, int out_f32) {
+  skinny_gemm_body<ROWS, NST, NB, false>(tmap_w, tmap_x, y, ldy, bias, resid, ldr, m, N, K, epi, out_f32, nullptr, 0);
+}
+
+// wsc: the fp32 scale of row n, k group j (k in [128 j, 128 j + 128)) at wsc[n * lds + j]
+template <int ROWS, int NST, int NB>
+__global__ void __launch_bounds__(SK2_THREADS)
+skinny_gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
+                       void* __restrict__ y, long long ldy, const bf16* __restrict__ bias,
+                       const bf16* __restrict__ resid, long long ldr, int m, int N, int K, int epi, int out_f32,
+                       const float* __restrict__ wsc, long long lds) {
+  skinny_gemm_body<ROWS, NST, NB, true>(tmap_w, tmap_x, y, ldy, bias, resid, ldr, m, N, K, epi, out_f32, wsc, lds);
+}
+
+// FP8 weights: W [N, K] bf16 -> E4M3 bytes q [N, K] (row stride ldq) and scales [N, K / 128] (row stride lds), one warp
+// per 128-value group under fp8_quant_row_warp (lane l: k 4l .. 4l + 3 of the group); and back, W-hat = float(q) * scale.
+__global__ void weight_quant_fp8_kernel(const bf16* __restrict__ w, long long ldw, uint8_t* __restrict__ q,
+                                        long long ldq, float* __restrict__ sc, long long lds, int N, int K) {
+  const int lane = threadIdx.x & 31, ng = K / 128;
+  const long long total = (long long)N * ng, stride = ((long long)gridDim.x * blockDim.x) >> 5;
+  for (long long gi = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; gi < total; gi += stride) {
+    const long long n = gi / ng;
+    const int j = (int)(gi % ng);
+    const uint2 raw = *reinterpret_cast<const uint2*>(w + n * ldw + j * 128 + 4 * lane);
+    const float2 f0 = unpack_bf16x2(raw.x), f1 = unpack_bf16x2(raw.y);
+    float x[4] = {f0.x, f0.y, f1.x, f1.y};
+    uint16_t q01, q23;
+    const float s = fp8_quant_row_warp(x, q01, q23);
+    *reinterpret_cast<uint32_t*>(q + n * ldq + j * 128 + 4 * lane) = (uint32_t)q01 | ((uint32_t)q23 << 16);
+    if (lane == 0) sc[n * lds + j] = s;
+  }
+}
+
+__global__ void weight_dequant_fp8_kernel(const uint8_t* __restrict__ q, long long ldq, const float* __restrict__ sc,
+                                          long long lds, bf16* __restrict__ w, long long ldw, int N, int K) {
+  const int lane = threadIdx.x & 31, ng = K / 128;
+  const long long total = (long long)N * ng, stride = ((long long)gridDim.x * blockDim.x) >> 5;
+  for (long long gi = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; gi < total; gi += stride) {
+    const long long n = gi / ng;
+    const int j = (int)(gi % ng);
+    const uint32_t u = *reinterpret_cast<const uint32_t*>(q + n * ldq + j * 128 + 4 * lane);
+    *reinterpret_cast<uint2*>(w + n * ldw + j * 128 + 4 * lane) = fp8x4_to_bf16x4(u, sc[n * lds + j]);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // decode attention (split-context). qkv: [B, (Hq+2Hkv)*128] (pre-RoPE); cache K/V: [B, Hkv, Tmax, 128].
 // grid (Hkv, B, S): every CTA handles 1/S of the cached positions of one (sequence, kv head) for the G
@@ -214,59 +299,7 @@ skinny_gemm_tma_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
 constexpr int DA_THREADS = 256;
 constexpr int DA_D = 128;
 
-// E4M3 row quantisation, one warp per 128-value row, 4 values per lane (any assignment of values to lanes). a = max |x|;
-// e = the least integer with a <= 448 * 2^e, at least -124 (so every float(q) * 2^e is a bf16 value and 2^e an fp32
-// normal); q = RNE_e4m3(x * 2^-e) (exact multiply, |x * 2^-e| <= 448: nothing saturates), except that at e = 120, the
-// largest e a bf16 row reaches, an entry that rounds to 256 (|x| >= 1.9375 * 2^127) would dequantise to 2^128, past the
-// bf16 and fp32 range: it stores 240 (0x77), the largest magnitude whose float(q) * 2^e is finite. A zero row stores
-// zeros with e = 0; a row holding any Inf or NaN stores the E4M3 NaN 0x7f everywhere with e = 0. On return x holds
-// float(q) * 2^e, q01 / q23 the bytes of (x[0], x[1]) and (x[2], x[3]) (first value in the low byte); returns 2^e.
-__device__ __forceinline__ uint16_t fp8x2_cap_256(uint16_t q) {
-  const uint16_t lo = (q & 0x7f) == 0x78 ? (q & 0x80) | 0x77 : q & 0xff;
-  const uint16_t hi = ((q >> 8) & 0x7f) == 0x78 ? ((q >> 8) & 0x80) | 0x77 : q >> 8;
-  return (uint16_t)(lo | (hi << 8));
-}
-
-__device__ __forceinline__ float fp8_quant_row_warp(float (&x)[4], uint16_t& q01, uint16_t& q23) {
-  float a = 0.f;
-  bool bad = false;
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float m = fabsf(x[j]);
-    bad |= !(m <= 3.402823466e38f);
-    a = fmaxf(a, m);
-  }
-  a = warp_max(a);
-  bad = __any_sync(0xffffffffu, bad);
-  int e = 0;
-  if (!bad && a > 0.f) {
-    int E;
-    const float f = frexpf(a, &E);          // a = f 2^E, f in [0.5, 1); 448 = 0.875 * 2^9
-    e = max(f <= 0.875f ? E - 9 : E - 8, -124);
-  }
-  const float sc = __int_as_float((127 + e) << 23), inv = __int_as_float((127 - e) << 23);
-  if (bad) {
-    q01 = q23 = 0x7f7f;
-  } else {
-    q01 = __nv_cvt_float2_to_fp8x2(make_float2(x[0] * inv, x[1] * inv), __NV_SATFINITE, __NV_E4M3);
-    q23 = __nv_cvt_float2_to_fp8x2(make_float2(x[2] * inv, x[3] * inv), __NV_SATFINITE, __NV_E4M3);
-    if (e == 120) {
-      q01 = fp8x2_cap_256(q01);
-      q23 = fp8x2_cap_256(q23);
-    }
-  }
-  const float2 d01 = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2(q01, __NV_E4M3)));
-  const float2 d23 = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2(q23, __NV_E4M3)));
-  x[0] = d01.x * sc; x[1] = d01.y * sc; x[2] = d23.x * sc; x[3] = d23.y * sc;
-  return sc;
-}
-
-// four E4M3 values (first in the low byte) -> float(q) * sc
-__device__ __forceinline__ void fp8x4_dequant(uint32_t u, float sc, float* f) {
-  const float2 a = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(u & 0xffffu), __NV_E4M3)));
-  const float2 b = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(u >> 16), __NV_E4M3)));
-  f[0] = a.x * sc; f[1] = a.y * sc; f[2] = b.x * sc; f[3] = b.y * sc;
-}
+// The E4M3 row rule (fp8_quant_row_warp, fp8x4_dequant) lives in fp8.cuh, shared with the FP8 weights.
 
 template <int G, bool PAGED, bool FP8 = false>
 __global__ void __launch_bounds__(DA_THREADS)
@@ -756,35 +789,55 @@ __global__ void decode_select_hidden_kernel(const int* __restrict__ mode, const 
 
 namespace {
 
-template <int ROWS, int NST, int NB>
+template <int ROWS, int NST, int NB, bool FP8>
 int launch_skinny_tma(const CUtensorMap& tw, const CUtensorMap& tx, void* y, long long ldy, const void* bias,
                       const void* resid, long long ldr, int m, int N, int K, int epilogue, int out_f32,
-                      cudaStream_t stream) {
-  constexpr int smem = NST * (4 * ROWS * 128 + 4 * 8 * NB * 128) + ((2 * NST * 8 + 127) & ~127) + 4 * ROWS * 8 * NB * 4 + 1024;
+                      const float* wsc, long long lds, cudaStream_t stream) {
+  constexpr int smem = NST * ((FP8 ? 2 : 4) * ROWS * 128 + 4 * 8 * NB * 128) + ((2 * NST * 8 + 127) & ~127) +
+                       4 * ROWS * 8 * NB * 4 + 1024;
   static_assert(smem <= 227 * 1024, "skinny GEMM ring does not fit in shared memory");
   static std::once_flag once;
   static cudaError_t err = cudaSuccess;
-  std::call_once(once, [&] {
-    err = cudaFuncSetAttribute(skinny_gemm_tma_kernel<ROWS, NST, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  });
-  MM_CHECK_CUDA(err);
-  MM_CHECK_CUDA(launch_pdl(skinny_gemm_tma_kernel<ROWS, NST, NB>, dim3((N + ROWS - 1) / ROWS), dim3(SK2_THREADS), smem,
-                           stream, tw, tx, y, ldy, (const bf16*)bias, (const bf16*)resid, ldr, m, N, K, epilogue, out_f32));
+  if constexpr (FP8) {
+    std::call_once(once, [&] {
+      err = cudaFuncSetAttribute(skinny_gemm_fp8_kernel<ROWS, NST, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    });
+    MM_CHECK_CUDA(err);
+    MM_CHECK_CUDA(launch_pdl(skinny_gemm_fp8_kernel<ROWS, NST, NB>, dim3((N + ROWS - 1) / ROWS), dim3(SK2_THREADS), smem,
+                             stream, tw, tx, y, ldy, (const bf16*)bias, (const bf16*)resid, ldr, m, N, K, epilogue,
+                             out_f32, wsc, lds));
+  } else {
+    std::call_once(once, [&] {
+      err = cudaFuncSetAttribute(skinny_gemm_tma_kernel<ROWS, NST, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    });
+    MM_CHECK_CUDA(err);
+    MM_CHECK_CUDA(launch_pdl(skinny_gemm_tma_kernel<ROWS, NST, NB>, dim3((N + ROWS - 1) / ROWS), dim3(SK2_THREADS), smem,
+                             stream, tw, tx, y, ldy, (const bf16*)bias, (const bf16*)resid, ldr, m, N, K, epilogue,
+                             out_f32));
+  }
   MM_CHECK_LAUNCH();
   return MM_OK;
 }
 
-}  // namespace
-
-MM_API int mm_skinny_gemm(const void* x, const void* W, void* y, const void* bias, const void* resid,
-                          long long ldx, long long ldw, long long ldy, long long ldr, int m, int N,
-                          int K, int epilogue, int out_f32, cudaStream_t stream) {
-  MM_CHECK_ARG(m >= 1 && m <= 32, "mm_skinny_gemm: batch must be in [1,32] (m=%d)", m);
-  MM_CHECK_ARG(K % 32 == 0 && ldx % 8 == 0 && ldw % 8 == 0, "mm_skinny_gemm: need K%%32==0, ldx/ldw%%8==0");
-  MM_CHECK_ARG(((uintptr_t)W & 15) == 0 && ((uintptr_t)x & 15) == 0, "mm_skinny_gemm: x / W must be 16-byte aligned");
-  MM_CHECK_ARG(epilogue >= SK_STORE && epilogue <= SK_SWIGLU, "mm_skinny_gemm: bad epilogue");
-  MM_CHECK_ARG((epilogue != SK_BIAS && epilogue != SK_BIAS_GELU) || bias, "mm_skinny_gemm: bias missing");
-  MM_CHECK_ARG(epilogue != SK_RESID || resid, "mm_skinny_gemm: residual missing");
+// mm_skinny_gemm and mm_skinny_gemm_fp8: argument checks, tensor maps and the slab / batch-tile dispatch; `name` prefixes
+// the error messages. FP8: W holds E4M3 bytes (ldw in bytes) and wsc the scales.
+template <bool FP8>
+int skinny_gemm_launch(const char* name, const void* x, const void* W, const float* wsc, void* y, const void* bias,
+                       const void* resid, long long ldx, long long ldw, long long lds, long long ldy, long long ldr,
+                       int m, int N, int K, int epilogue, int out_f32, cudaStream_t stream) {
+  MM_CHECK_ARG(m >= 1 && m <= 32, "%s: batch must be in [1,32] (m=%d)", name, m);
+  if constexpr (FP8) {
+    MM_CHECK_ARG(K >= 128 && K % 128 == 0 && ldx % 8 == 0 && ldw % 16 == 0 && ldw >= K,
+                 "%s: need K%%128==0, ldx%%8==0, ldw%%16==0 and ldw>=K", name);
+    MM_CHECK_ARG(wsc != nullptr && lds >= K / 128, "%s: scales missing or lds < K/128", name);
+    MM_CHECK_ARG(((uintptr_t)wsc & 3) == 0, "%s: scales must be 4-byte aligned", name);
+  } else {
+    MM_CHECK_ARG(K % 32 == 0 && ldx % 8 == 0 && ldw % 8 == 0, "%s: need K%%32==0, ldx/ldw%%8==0", name);
+  }
+  MM_CHECK_ARG(((uintptr_t)W & 15) == 0 && ((uintptr_t)x & 15) == 0, "%s: x / W must be 16-byte aligned", name);
+  MM_CHECK_ARG(epilogue >= SK_STORE && epilogue <= SK_SWIGLU, "%s: bad epilogue", name);
+  MM_CHECK_ARG((epilogue != SK_BIAS && epilogue != SK_BIAS_GELU) || bias, "%s: bias missing", name);
+  MM_CHECK_ARG(epilogue != SK_RESID || resid, "%s: residual missing", name);
   // The batch is the n dimension of the MMA: 1, 2 or 4 n8 tiles (8 / 16 / 32 sequences) share every weight fragment.
   const int nb = m <= 8 ? 1 : (m <= 16 ? 2 : 4);
   // 32-row slabs where the epilogue needs them (SwiGLU: 16 gate + 16 up rows of the same channels), for very large N
@@ -794,7 +847,7 @@ MM_API int mm_skinny_gemm(const void* x, const void* W, void* y, const void* bia
   // 32 sequences, wide outputs (gate/up, lm_head): 64-row slabs halve the L2 -> SM activation traffic again, which at this
   // batch equals the weight stream and caps the kernel (measured 4.1 TB/s of weights + as much of x with 32-row slabs)
   const bool rows64 = nb == 4 && N >= 64 * 2 * mm_num_sms() && (epilogue != SK_SWIGLU || N % 64 == 0);
-  if (epilogue == SK_SWIGLU) MM_CHECK_ARG(N % 32 == 0 && !out_f32, "mm_skinny_gemm: SWIGLU needs N%%32==0");
+  if (epilogue == SK_SWIGLU) MM_CHECK_ARG(N % 32 == 0 && !out_f32, "%s: SWIGLU needs N%%32==0", name);
   static PFN_encodeTiledSk enc = nullptr;
   static std::once_flag once;
   std::call_once(once, [] {
@@ -804,17 +857,18 @@ MM_API int mm_skinny_gemm(const void* x, const void* W, void* y, const void* bia
         q == cudaDriverEntryPointSuccess)
       enc = reinterpret_cast<PFN_encodeTiledSk>(fn);
   });
-  MM_CHECK_ARG(enc != nullptr, "mm_skinny_gemm: cuTensorMapEncodeTiled unavailable");
+  MM_CHECK_ARG(enc != nullptr, "%s: cuTensorMapEncodeTiled unavailable", name);
   CUtensorMap tw, tx;
   cuuint32_t estr[2] = {1, 1};
   {
+    // bf16: [rows x 64 k] boxes; FP8: [rows x 128 k] uint8 boxes. Either way one 128-byte swizzled row per weight row.
     cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)N};
-    cuuint64_t strides[1] = {(cuuint64_t)ldw * 2};
-    cuuint32_t box[2] = {64, (cuuint32_t)(rows64 ? 64 : (rows32 ? 32 : 16))};
-    CUresult r = enc(&tw, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(W), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    MM_CHECK_ARG(r == CUDA_SUCCESS, "mm_skinny_gemm: cuTensorMapEncodeTiled(W) failed (%d)", (int)r);
+    cuuint64_t strides[1] = {(cuuint64_t)ldw * (FP8 ? 1 : 2)};
+    cuuint32_t box[2] = {FP8 ? 128u : 64u, (cuuint32_t)(rows64 ? 64 : (rows32 ? 32 : 16))};
+    CUresult r = enc(&tw, FP8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(W),
+                     dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    MM_CHECK_ARG(r == CUDA_SUCCESS, "%s: cuTensorMapEncodeTiled(W) failed (%d)", name, (int)r);
   }
   {
     cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)m};            // rows >= m of the box are zero-filled
@@ -823,20 +877,86 @@ MM_API int mm_skinny_gemm(const void* x, const void* W, void* y, const void* bia
     CUresult r = enc(&tx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(x), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    MM_CHECK_ARG(r == CUDA_SUCCESS, "mm_skinny_gemm: cuTensorMapEncodeTiled(x) failed (%d)", (int)r);
+    MM_CHECK_ARG(r == CUDA_SUCCESS, "%s: cuTensorMapEncodeTiled(x) failed (%d)", name, (int)r);
   }
   // Ring depths: as deep as keeps two CTAs per SM (profiles/r02_decode_skinny_ring_sweep.txt: deeper rings bought nothing);
-  // 32 sequences: 32 KB (32-row slabs) or 48 KB (64-row slabs) stages, one CTA per SM.
-#define MM_SK(R, S, B) return launch_skinny_tma<R, S, B>(tw, tx, y, ldy, bias, resid, ldr, m, N, K, epilogue, out_f32, stream)
-  if (rows64) MM_SK(64, 4, 4);
-  if (nb == 4) MM_SK(32, 5, 4);
-  if (nb == 2) {
-    if (rows32) MM_SK(32, 4, 2);
-    MM_SK(16, 6, 2);
+  // 32 sequences: 32 KB (32-row slabs) or 48 KB (64-row slabs) stages, one CTA per SM. An FP8 stage carries half the
+  // weight bytes of a bf16 one, so its ring is deeper in the same shared memory.
+#define MM_SK(R, S, B) \
+  return launch_skinny_tma<R, S, B, FP8>(tw, tx, y, ldy, bias, resid, ldr, m, N, K, epilogue, out_f32, wsc, lds, stream)
+  if constexpr (FP8) {
+    if (rows64) MM_SK(64, 6, 4);
+    if (nb == 4) MM_SK(32, 6, 4);
+    if (nb == 2) {
+      if (rows32) MM_SK(32, 6, 2);
+      MM_SK(16, 8, 2);
+    }
+    if (rows32) MM_SK(32, 8, 1);
+    MM_SK(16, 12, 1);
+  } else {
+    if (rows64) MM_SK(64, 4, 4);
+    if (nb == 4) MM_SK(32, 5, 4);
+    if (nb == 2) {
+      if (rows32) MM_SK(32, 4, 2);
+      MM_SK(16, 6, 2);
+    }
+    if (rows32) MM_SK(32, 5, 1);
+    MM_SK(16, 8, 1);
   }
-  if (rows32) MM_SK(32, 5, 1);
-  MM_SK(16, 8, 1);
 #undef MM_SK
+}
+
+}  // namespace
+
+MM_API int mm_skinny_gemm(const void* x, const void* W, void* y, const void* bias, const void* resid,
+                          long long ldx, long long ldw, long long ldy, long long ldr, int m, int N,
+                          int K, int epilogue, int out_f32, cudaStream_t stream) {
+  return skinny_gemm_launch<false>("mm_skinny_gemm", x, W, nullptr, y, bias, resid, ldx, ldw, 0, ldy, ldr, m, N, K,
+                                   epilogue, out_f32, stream);
+}
+
+MM_API int mm_skinny_gemm_fp8(const void* x, const void* Wq, const float* wscale, void* y, const void* bias,
+                              const void* resid, long long ldx, long long ldw, long long lds, long long ldy,
+                              long long ldr, int m, int N, int K, int epilogue, int out_f32, cudaStream_t stream) {
+  return skinny_gemm_launch<true>("mm_skinny_gemm_fp8", x, Wq, wscale, y, bias, resid, ldx, ldw, lds, ldy, ldr, m, N, K,
+                                  epilogue, out_f32, stream);
+}
+
+namespace {
+
+int weight_fp8_check(const char* name, const void* a, const void* b, const void* sc, long long lda, long long ldb,
+                     long long lds, int N, int K) {
+  MM_CHECK_ARG(a != nullptr && b != nullptr && sc != nullptr, "%s: null pointer", name);
+  MM_CHECK_ARG(N >= 1 && K >= 128 && K % 128 == 0, "%s: need N>=1 and K a positive multiple of 128 (N=%d K=%d)", name,
+               N, K);
+  MM_CHECK_ARG(lda >= K && ldb >= K && lds >= K / 128 && lda % 4 == 0 && ldb % 4 == 0,
+               "%s: need row strides >= K (multiples of 4) and lds >= K/128", name);
+  MM_CHECK_ARG((((uintptr_t)a | (uintptr_t)b) & 7) == 0 && ((uintptr_t)sc & 3) == 0, "%s: misaligned operand", name);
+  return MM_OK;
+}
+
+}  // namespace
+
+MM_API int mm_weight_quant_fp8(const void* W, long long ldw, void* q, long long ldq, float* scale, long long lds, int N,
+                               int K, cudaStream_t stream) {
+  const int rc = weight_fp8_check("mm_weight_quant_fp8", W, q, scale, ldw, ldq, lds, N, K);
+  if (rc != MM_OK) return rc;
+  long long blocks = ceil_div64((long long)N * (K / 128) * 32, 256);
+  if (blocks > (long long)mm_num_sms() * 16) blocks = (long long)mm_num_sms() * 16;
+  weight_quant_fp8_kernel<<<(int)blocks, 256, 0, stream>>>((const bf16*)W, ldw, (uint8_t*)q, ldq, scale, lds, N, K);
+  MM_CHECK_LAUNCH();
+  return MM_OK;
+}
+
+MM_API int mm_weight_dequant_fp8(const void* q, long long ldq, const float* scale, long long lds, void* W,
+                                 long long ldw, int N, int K, cudaStream_t stream) {
+  const int rc = weight_fp8_check("mm_weight_dequant_fp8", q, W, scale, ldq, ldw, lds, N, K);
+  if (rc != MM_OK) return rc;
+  long long blocks = ceil_div64((long long)N * (K / 128) * 32, 256);
+  if (blocks > (long long)mm_num_sms() * 16) blocks = (long long)mm_num_sms() * 16;
+  weight_dequant_fp8_kernel<<<(int)blocks, 256, 0, stream>>>((const uint8_t*)q, ldq, scale, lds, (bf16*)W, ldw, N, K);
+  MM_CHECK_LAUNCH();
+  return MM_OK;
 }
 
 MM_API long long mm_decode_attn_workspace_bytes(int B, int Hq, int Hkv, int splits) {

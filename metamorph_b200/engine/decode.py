@@ -15,6 +15,7 @@ import torch
 from .. import ops
 from ..constants import EOS_TOKEN_IDS, IMAGE_END_TOKEN_ID, IMAGE_START_TOKEN_ID
 from .decode_step import decode_heads, decoder_stack_step
+from .fp8_weights import decode_weights
 from .llama import FP8KVStore, StackContext
 from .logprobs import LogprobBuffers, check_logprobs
 from .sampling import SamplingArrays, SamplingParams, per_sequence
@@ -44,6 +45,16 @@ def check_kv_cache_dtype(kv_cache_dtype) -> None:
         raise ValueError(f"kv_cache_dtype must be one of {KV_CACHE_DTYPES} (got {kv_cache_dtype!r})")
 
 
+WEIGHT_DTYPES = ("bf16", "fp8_e4m3")
+
+
+def check_weight_dtype(weight_dtype) -> None:
+    """'bf16' (the model's parameters) or 'fp8_e4m3' (the decode step streams E4M3 weight groups with one power-of-two
+    scale per 128 k, DESIGN.md §1). Raises ValueError on the host, before any device work."""
+    if not isinstance(weight_dtype, str) or weight_dtype not in WEIGHT_DTYPES:
+        raise ValueError(f"weight_dtype must be one of {WEIGHT_DTYPES} (got {weight_dtype!r})")
+
+
 def alloc_kv_cache(kv_cache_dtype: str, shape, dev):
     """(kc, vc, scales) for a cache of `shape` [..., dh]: bf16 and scales None, or uint8 E4M3 bytes and (ks, vs) fp32
     [...] (one scale per row). Zero-filled."""
@@ -67,7 +78,7 @@ class DecodeEngine:
                  forced_tokens: Optional[torch.Tensor] = None, poll_every: int = 16,
                  max_steps: Optional[int] = None,
                  sampling: Union[None, SamplingParams, Sequence[SamplingParams]] = None,
-                 logprobs: Optional[int] = None, kv_cache_dtype: str = "bf16"):
+                 logprobs: Optional[int] = None, kv_cache_dtype: str = "bf16", weight_dtype: str = "bf16"):
         """inputs_embeds [B, P, H] (right-padded to P; prompt_lens[b] valid rows). B <= 128.
         sampling: None (greedy), one SamplingParams (sequence b draws with seed + b) or one per sequence. The draw
         replaces the argmax only: image mode, the EOS test on the drawn token and forced tokens are unchanged. When
@@ -83,10 +94,16 @@ class DecodeEngine:
         (half the bytes), and every attention, prefill and decode, reads the values the cache holds. Right-padded
         prompts quantise their pad rows like any other row; nothing reads them. Anything else raises ValueError before
         any device work.
+        weight_dtype: 'bf16' (default) or 'fp8_e4m3': the call first quantises the decoder-layer matrices and lm_head
+        into E4M3 groups (engine/fp8_weights.py; about 1.03 bytes per parameter, beside the bf16 parameters, plus one
+        layer of bf16 scratch) and the decode steps stream those, about half the bytes. The prefill dequantises them
+        layer by layer, so the run returns the bits of the bf16 path on a model holding W-hat. The quantisation time is
+        `last_timing['quant_ms']`, outside 'decode_ms'. Anything else raises ValueError before any device work.
         Returns (ids list per sequence (int32 tensors), image_embeds list per sequence [n, C]), and with logprobs a
         third element: one TokenLogprobs per sequence, entry k belonging to ids[k]."""
         check_logprobs(logprobs)
         check_kv_cache_dtype(kv_cache_dtype)
+        check_weight_dtype(weight_dtype)
         B, P, H = inputs_embeds.shape
         assert B <= 128, f"decode batch is limited to 128 sequences per step (got {B}): the weight-streaming GEMM " \
                          "serves at most 128 batch rows"
@@ -116,14 +133,19 @@ class DecodeEngine:
         eos0 = eos[0] if eos else -1
         eos1 = eos[1] if len(eos) > 1 else eos0
 
+        qev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+        qev[0].record()
+        dw = decode_weights(m, weight_dtype)
+        qev[1].record()
         kc, vc, scales = alloc_kv_cache(kv_cache_dtype, (L, B, Hkv, Tmax, dh), dev)
 
         # ---- prefill: full-sequence kernels, K/V captured into the cache
         pos = torch.arange(P, dtype=torch.int32).repeat(B).to(dev)
         ctx = StackContext(B=B, T=P, pos=pos, seqlens=prompt_lens_dev)
-        layers = [l.weights() for l in model.layers]
+        layers = dw.layers
         x = inputs_embeds.reshape(B * P, H).contiguous()
-        for i, w in enumerate(layers):
+        for i in range(L):
+            w = dw.prefill_layer(i)
             if scales is not None:
                 x = stack.layer_forward(w, x, ctx, save=True, save_gu=False,
                                         kv=FP8KVStore(kc[i], vc[i], scales[0][i], scales[1][i]))
@@ -156,7 +178,7 @@ class DecodeEngine:
 
         def heads_and_state(h_pre_norm, step):
             tok, pred_z, prediction = decode_heads(m, h_pre_norm, st["in_image_mode"], logits, V, samp,
-                                                   st["total_output"])
+                                                   st["total_output"], dw.lm_head)
             ops.decode_state_step(st, tok, forced, step, B, ntok, max_new_tokens, start_image_token_id,
                                   end_image_token_id, eos0, eos1, pred_z, img_out)
             if lpb is not None:
@@ -211,7 +233,8 @@ class DecodeEngine:
         self.last_steps = step
         # device time of the decode steps (graph capture is a one-off host-side cost, reported separately)
         self.last_timing = {"steps": step, "decode_ms": ev[0].elapsed_time(ev[1]) + ev[2].elapsed_time(ev[3]),
-                            "capture_ms": ev[1].elapsed_time(ev[2]), "cuda_graph": graph is not None}
+                            "capture_ms": ev[1].elapsed_time(ev[2]), "cuda_graph": graph is not None,
+                            "quant_ms": qev[0].elapsed_time(qev[1])}
         if lpb is not None:
             return out_ids, out_img, [lpb.take(b, 0, n_ids[b], int(logprobs)) for b in range(B)]
         return out_ids, out_img

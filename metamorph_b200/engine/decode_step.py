@@ -14,7 +14,8 @@ def decoder_stack_step(layers, x, kc, vc, cur_pos, stack, table=None, scales=Non
     With a block table [B, max_blocks] (int32, device) kc/vc are paged pools [L, num_blocks, Hkv, block_size, dh] and
     the attention addresses them through it (ops.decode_attn_paged: the same bits as the dense cache).
     scales: None (bf16 cache), or the (ks, vs) fp32 scale arrays of an FP8 cache ([L, B, Hkv, Tmax] dense, [L,
-    num_blocks, Hkv, block_size] paged; kc/vc are then uint8 E4M3 bytes) for the FP8 attention kernels."""
+    num_blocks, Hkv, block_size] paged; kc/vc are then uint8 E4M3 bytes) for the FP8 attention kernels.
+    The four matrices of a layer may be ops.FP8Weights (engine/fp8_weights.py): skinny_gemm streams them as E4M3."""
     d = stack.dims
     Hq, Hkv, dh = d.n_heads, d.n_kv_heads, d.head_dim
     for i, w in enumerate(layers):
@@ -38,9 +39,10 @@ def decoder_stack_step(layers, x, kc, vc, cur_pos, stack, table=None, scales=Non
     return x
 
 
-def decode_heads(m, h_pre_norm, in_image_mode, logits, V, sampling=None, counter=None):
+def decode_heads(m, h_pre_norm, in_image_mode, logits, V, sampling=None, counter=None, lm_head=None):
     """-> (token [B] int32, pred_z [B, C] (normalised visual embedding), prediction [B, H] (its projection)).
     The image-mode branch is computed for every sequence and selected per sequence (graph friendly).
+    lm_head: None (the model's bf16 parameter) or the weight to stream instead, e.g. its ops.FP8Weight.
     sampling: None = argmax (metamorph_llama.py:542); else a SamplingArrays of per-row device parameters, and the token
     is the seeded draw of ops.sample_rows with `counter` [B] int32 (steps each sequence has taken) on the device."""
     inner = m.get_model()
@@ -54,7 +56,7 @@ def decode_heads(m, h_pre_norm, in_image_mode, logits, V, sampling=None, counter
     prediction = ops.skinny_gemm(p1, pj.fc2.weight.data, bias=pj.fc2.bias.data, epilogue=ops.SK_BIAS)
     h_eff = torch.empty_like(hidden)
     ops.decode_select_hidden(in_image_mode, hidden, prediction, h_eff)
-    ops.skinny_gemm(h_eff, m.lm_head.weight.data, out=logits[:, :V])
+    ops.skinny_gemm(h_eff, m.lm_head.weight.data if lm_head is None else lm_head, out=logits[:, :V])
     if sampling is None:
         tok = ops.argmax_rows(logits, V)
     else:

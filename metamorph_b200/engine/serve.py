@@ -28,6 +28,9 @@ bytes of bf16: every prefill quantises its K/V into the cache before its attenti
 values, and the decode step runs the FP8 attention kernels. A prefixed prefill dequantises the shared blocks into a
 per-server bf16 staging pool and attends there. A row's bytes depend on that row alone, so paged equals dense, a prefixed
 request equals its whole prompt and a request does not depend on its neighbours, exactly as on a bf16 server.
+With `weight_dtype="fp8_e4m3"` the server quantises the decoder-layer matrices and lm_head into E4M3 groups once, in its
+constructor (engine/fp8_weights.py), and every step streams those; every prefill dequantises them one layer at a time
+into a bf16 scratch layer. A request returns the bits it would return from a bf16 server on a model holding W-hat.
 A request may ask for token log-probabilities (`submit(..., logprobs=n)`): while one is in flight the step runs a graph
 that adds the logprob kernel after the state step (captured the first time it is needed, for the greedy and the sampled
 step alike); its slot's `n_top` is written on admission, -1 for every request that did not ask. The kernel only reads
@@ -45,8 +48,9 @@ import torch
 
 from .. import ops
 from ..constants import EOS_TOKEN_IDS, IMAGE_END_TOKEN_ID, IMAGE_START_TOKEN_ID
-from .decode import alloc_kv_cache, check_forced_tokens, check_kv_cache_dtype
+from .decode import alloc_kv_cache, check_forced_tokens, check_kv_cache_dtype, check_weight_dtype
 from .decode_step import decode_heads, decoder_stack_step
+from .fp8_weights import decode_weights
 from .llama import FP8KVStore, PagedPrefill, StackContext
 from .logprobs import LogprobBuffers, TokenLogprobs, cat as cat_logprobs, check_logprobs
 from .sampling import SamplingArrays, SamplingParams
@@ -165,15 +169,21 @@ class ContinuousBatcher:
     def __init__(self, model, max_slots: int = 8, max_context: int = 2048, max_new_tokens: int = 1024,
                  poll_every: int = 8, use_cuda_graph: bool = True, start_image_token_id: int = IMAGE_START_TOKEN_ID,
                  end_image_token_id: int = IMAGE_END_TOKEN_ID, eos_token_id=EOS_TOKEN_IDS,
-                 kv_pool_tokens: Optional[int] = None, kv_block_size: int = 64, kv_cache_dtype: str = "bf16"):
+                 kv_pool_tokens: Optional[int] = None, kv_block_size: int = 64, kv_cache_dtype: str = "bf16",
+                 weight_dtype: str = "bf16"):
         """kv_pool_tokens: None keeps one dense cache region of max_context positions per slot. An integer gives a
         paged cache: a pool of ceil(kv_pool_tokens / kv_block_size) blocks (plus one scratch block) shared by all
         slots; a request is admitted (strictly first come, first served) once a slot and the blocks it needs
         are free. max_context stays the longest request either way.
         kv_cache_dtype: 'bf16' or 'fp8_e4m3' (E4M3 rows + one fp32 scale per row: 1 byte per element plus 4 per row, so
         a pool of the same bytes holds about 1.94x the positions; kv_pool_tokens still counts positions). Anything else
-        raises ValueError before any device work."""
+        raises ValueError before any device work.
+        weight_dtype: 'bf16' or 'fp8_e4m3': the decoder-layer matrices and lm_head are quantised here, once, into E4M3
+        groups the decode step streams (about half the bytes per step). They are a snapshot, like the bf16 layer list:
+        later changes to the parameters are not seen. The FP8 copy (about 1.03 bytes per parameter) and one layer of bf16
+        scratch live beside the model's bf16 parameters. Anything else raises ValueError before any device work."""
         check_kv_cache_dtype(kv_cache_dtype)
+        check_weight_dtype(weight_dtype)
         assert 1 <= max_slots <= 128, f"the weight-streaming step serves at most 128 sequences (max_slots={max_slots})"
         check_kv_block_size(kv_block_size)
         if kv_pool_tokens is not None and (not isinstance(kv_pool_tokens, int) or kv_pool_tokens < 1):
@@ -188,7 +198,9 @@ class ContinuousBatcher:
         self.dev = self.inner.embed_tokens.weight.device
         dev, B = self.dev, max_slots
         self.L = len(self.inner.layers)
-        self.layers = [l.weights() for l in self.inner.layers]
+        self.weight_dtype = weight_dtype
+        self.weights = decode_weights(model, weight_dtype)
+        self.layers = self.weights.layers
         self.ntok = model.get_vision_tower().image_token_len if model.get_vision_tower() is not None else 0
         self.C = model.vision_head.fc2.out_features
         eos = list(eos_token_id) if isinstance(eos_token_id, (list, tuple)) else [eos_token_id]
@@ -255,7 +267,7 @@ class ContinuousBatcher:
         x = decoder_stack_step(self.layers, self.xin, self.kc, self.vc, st["pos"] - 1, self.stack, self.table,
                                self.scales)
         tok, pred_z, prediction = decode_heads(self.m, x, st["in_image_mode"], self.logits, self.V,
-                                               self.samp if sampled else None, st["total_output"])
+                                               self.samp if sampled else None, st["total_output"], self.weights.lm_head)
         ops.decode_state_step_slots(st, tok, self.forced, self.max_new_slot, self.B, self.ntok, self.start_id,
                                     self.end_id, self.eos0, self.eos1, pred_z, self.img_out)
         if logprobs:
@@ -395,7 +407,8 @@ class ContinuousBatcher:
         row = torch.tensor(blocks, dtype=torch.int32).to(self.dev)
         ctx = StackContext(B=1, T=Ls, pos=torch.arange(Ls, dtype=torch.int32, device=self.dev), seqlens=None)
         x = e[:Ls]
-        for i, w in enumerate(self.layers):
+        for i in range(self.L):
+            w = self.weights.prefill_layer(i)
             if self.scales is not None:
                 x = self.stack.layer_forward(w, x, ctx, save=True, save_gu=False,
                                              kv=FP8KVStore(self.kc[i], self.vc[i], self.scales[0][i],
@@ -437,7 +450,8 @@ class ContinuousBatcher:
                 pos = torch.arange(Ls, Ls + P - 1, dtype=torch.int32, device=self.dev)
                 ctx = StackContext(B=1, T=P - 1, pos=pos, seqlens=None)
                 x = req.embeds[:P - 1].contiguous()
-                for i, w in enumerate(self.layers):
+                for i in range(self.L):
+                    w = self.weights.prefill_layer(i)
                     if self.scales is not None:
                         x = self.stack.layer_forward(w, x, ctx, save=False, save_gu=False,
                                                      kv=FP8KVStore(self.kc[i], self.vc[i], self.scales[0][i],
@@ -450,7 +464,8 @@ class ContinuousBatcher:
             pos = torch.arange(P - 1, dtype=torch.int32, device=self.dev)
             ctx = StackContext(B=1, T=P - 1, pos=pos, seqlens=None)
             x = req.embeds[:P - 1].contiguous()
-            for i, w in enumerate(self.layers):
+            for i in range(self.L):
+                w = self.weights.prefill_layer(i)
                 if self.scales is not None:
                     ks, vs = self.scales[0][i], self.scales[1][i]
                     kv = FP8KVStore(self.kc[i, b:b + 1], self.vc[i, b:b + 1], ks[b:b + 1], vs[b:b + 1]) \

@@ -26,7 +26,7 @@ import torch.nn as nn
 
 from .. import ops
 from ..constants import EOS_TOKEN_IDS, IGNORE_INDEX, IMAGE_END_TOKEN_ID, IMAGE_START_TOKEN_ID, VISION_FEATURE_DIM
-from ..engine.decode import DecodeEngine, check_kv_cache_dtype
+from ..engine.decode import DecodeEngine, check_kv_cache_dtype, check_weight_dtype
 from ..engine.logprobs import check_logprobs
 from ..engine.hot_path import GradProvider, HotPath
 from ..engine.llama import LlamaDims, LlamaStack, StackContext
@@ -428,7 +428,8 @@ class MetaMorphLlamaForCausalLM(nn.Module, MetaMorphMetaForCausalLM):
                       start_image_token_id=IMAGE_START_TOKEN_ID, end_image_token_id=IMAGE_END_TOKEN_ID,
                       eos_token_id=list(EOS_TOKEN_IDS), do_sample=None, temperature=None, top_p=None,
                       num_beams=None, max_new_tokens=1024, use_cache=None, output_image=False,
-                      prompt_lens=None, forced_tokens=None, sampling=None, logprobs=None, kv_cache_dtype="bf16"):
+                      prompt_lens=None, forced_tokens=None, sampling=None, logprobs=None, kv_cache_dtype="bf16",
+                      weight_dtype="bf16"):
         """metamorph_llama.py:502-597 with a KV cache; accepts a batch (<= 8) of right-padded prompts.
         sampling: None (greedy, as the reference), a SamplingParams (sequence b draws with seed + b) or one per
         sequence (metamorph_b200.engine.sampling). The seeded draw replaces the argmax of metamorph_llama.py:542 and
@@ -436,12 +437,14 @@ class MetaMorphLlamaForCausalLM(nn.Module, MetaMorphMetaForCausalLM):
         greedy_decode ignores them: sampling is asked for with `sampling=` only.
         logprobs: None, or an int n in [0, 20]: the list of TokenLogprobs per sequence (engine/logprobs.py) is appended
         as the last return element; without it the return convention is the reference's.
-        kv_cache_dtype: 'bf16' (default) or 'fp8_e4m3' (an E4M3 KV cache, DecodeEngine.generate)."""
+        kv_cache_dtype: 'bf16' (default) or 'fp8_e4m3' (an E4M3 KV cache, DecodeEngine.generate).
+        weight_dtype: 'bf16' (default) or 'fp8_e4m3' (the decode step streams E4M3 weight groups quantised at the start of
+        the call, DecodeEngine.generate; the bf16 parameters stay and are not changed)."""
         res = self._decode.generate(inputs_embeds, prompt_lens=prompt_lens, max_new_tokens=max_new_tokens,
                                     start_image_token_id=start_image_token_id,
                                     end_image_token_id=end_image_token_id, eos_token_id=eos_token_id,
                                     forced_tokens=forced_tokens, sampling=sampling, logprobs=logprobs,
-                                    kv_cache_dtype=kv_cache_dtype)
+                                    kv_cache_dtype=kv_cache_dtype, weight_dtype=weight_dtype)
         ids, imgs = res[0], res[1]
         B = inputs_embeds.shape[0]
         if B == 1:  # reference return convention: [ids] and a [n, 1152] tensor
@@ -462,6 +465,7 @@ class MetaMorphLlamaForCausalLM(nn.Module, MetaMorphMetaForCausalLM):
         `do_sample` / `temperature` / `top_p` are dropped on this custom-greedy path, as in the reference."""
         check_logprobs(kwargs.get("logprobs"))
         check_kv_cache_dtype(kwargs.get("kv_cache_dtype", "bf16"))
+        check_weight_dtype(kwargs.get("weight_dtype", "bf16"))
         position_ids = kwargs.pop("position_ids", None)
         attention_mask = kwargs.pop("attention_mask", None)
         prompt_lens = None

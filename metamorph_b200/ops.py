@@ -458,12 +458,84 @@ ctypes_ll = _ctypes.c_longlong
 SK_STORE, SK_BIAS, SK_RESID, SK_BIAS_GELU, SK_SWIGLU = range(5)
 
 
+FP8_GROUP = 128
+
+
+class FP8Weight:
+    """A weight matrix W [N, K] stored as E4M3 groups (DESIGN.md §1): q [N, K] uint8 bytes and scale [N, K / 128] fp32,
+    one power-of-two scale per 128 consecutive k of a row, under the FP8 KV cache's row rule. W-hat = float(q) * scale is
+    exact and a bf16 value (`weight_dequant_fp8`). Immutable; both tensors are contiguous and on one CUDA device."""
+
+    __slots__ = ("q", "scale")
+
+    def __init__(self, q: torch.Tensor, scale: torch.Tensor):
+        if not isinstance(q, torch.Tensor) or not isinstance(scale, torch.Tensor):
+            raise TypeError("FP8Weight(q, scale) takes two tensors")
+        if q.dtype != torch.uint8 or q.dim() != 2:
+            raise ValueError(f"FP8Weight: q must be a 2-D uint8 tensor of E4M3 bytes (got {q.dtype}, {q.dim()}-D)")
+        N, K = q.shape
+        if N < 1 or K < FP8_GROUP or K % FP8_GROUP:
+            raise ValueError(f"FP8Weight: K must be a positive multiple of {FP8_GROUP} (q is [{N}, {K}])")
+        if scale.dtype != torch.float32 or tuple(scale.shape) != (N, K // FP8_GROUP):
+            raise ValueError(f"FP8Weight: scale must be fp32 [{N}, {K // FP8_GROUP}] (got {scale.dtype} "
+                             f"{list(scale.shape)})")
+        if not (q.is_contiguous() and scale.is_contiguous()):
+            raise ValueError("FP8Weight: q and scale must be contiguous")
+        if q.device != scale.device:
+            raise ValueError(f"FP8Weight: q and scale on different devices ({q.device}, {scale.device})")
+        object.__setattr__(self, "q", q)
+        object.__setattr__(self, "scale", scale)
+
+    def __setattr__(self, name, value):
+        raise AttributeError("FP8Weight is immutable")
+
+    @property
+    def shape(self):
+        return self.q.shape
+
+    @property
+    def device(self):
+        return self.q.device
+
+    def __repr__(self):
+        return f"FP8Weight(shape={tuple(self.q.shape)}, device={self.q.device})"
+
+
+def weight_quant_fp8(w: torch.Tensor) -> FP8Weight:
+    """bf16 W [N, K] (K a multiple of 128, row-major) -> FP8Weight, one warp per 128-value group."""
+    require_cuda(w)
+    assert w.dtype == torch.bfloat16 and w.dim() == 2 and w.stride(1) == 1, "weight_quant_fp8: bf16 [N, K] row-major"
+    N, K = w.shape
+    if K < FP8_GROUP or K % FP8_GROUP:
+        raise ValueError(f"weight_quant_fp8: K must be a positive multiple of {FP8_GROUP} (got {K})")
+    q = torch.empty((N, K), dtype=torch.uint8, device=w.device)
+    sc = torch.empty((N, K // FP8_GROUP), dtype=torch.float32, device=w.device)
+    call("mm_weight_quant_fp8", ptr(w), ll(w.stride(0)), ptr(q), ll(K), ptr(sc), ll(K // FP8_GROUP), c_int(N), c_int(K),
+         stream_ptr())
+    return FP8Weight(q, sc)
+
+
+def weight_dequant_fp8(w: FP8Weight, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """FP8Weight -> W-hat = float(q) * scale, bf16 [N, K] (into `out`, a row-major bf16 [N, K] view, when given)."""
+    require_cuda(w.q, out)
+    N, K = w.q.shape
+    if out is None:
+        out = torch.empty((N, K), dtype=torch.bfloat16, device=w.q.device)
+    assert out.dtype == torch.bfloat16 and tuple(out.shape) == (N, K) and out.stride(1) == 1
+    call("mm_weight_dequant_fp8", ptr(w.q), ll(K), ptr(w.scale), ll(K // FP8_GROUP), ptr(out), ll(out.stride(0)),
+         c_int(N), c_int(K), stream_ptr())
+    return out
+
+
 def skinny_gemm(x, w, *, bias=None, resid=None, epilogue=SK_STORE, out=None, out_dtype=torch.bfloat16, wide=None):
     """y[m<=128, N] = x[m, K] w[N, K]^T — HBM-bound weight streaming for the decode step.
     m <= 32 runs `mm_skinny_gemm` (mma.sync, the batch is 1, 2 or 4 n8 tiles); 33 <= m <= 128 runs `mm_skinny_gemm_wide`
     (wgmma over a 128-wide batch operand, split-K reduced in a fixed order). The two agree within bf16 rounding; within one
-    kernel a row's bits do not depend on the other rows. `wide=True` forces the wide kernel for any m (comparisons)."""
-    require_cuda(x, w, bias, resid, out)
+    kernel a row's bits do not depend on the other rows. `wide=True` forces the wide kernel for any m (comparisons).
+    w may be an FP8Weight: the same choice runs `mm_skinny_gemm_fp8` / `mm_skinny_gemm_wide_fp8`, whose output bits are
+    the bf16 kernel's on W-hat (weight_dequant_fp8(w))."""
+    fp8 = isinstance(w, FP8Weight)
+    require_cuda(x, w.q if fp8 else w, bias, resid, out)
     m, K = x.shape
     N = w.shape[0]
     n_out = N // 2 if epilogue == SK_SWIGLU else N
@@ -471,6 +543,13 @@ def skinny_gemm(x, w, *, bias=None, resid=None, epilogue=SK_STORE, out=None, out
         wide = m > 32
     if out is None:
         out = torch.empty((m, n_out), dtype=out_dtype, device=x.device)
+    if fp8:
+        assert w.shape[1] == K, f"contraction mismatch {K} vs {w.shape[1]}"
+        call("mm_skinny_gemm_wide_fp8" if wide else "mm_skinny_gemm_fp8", ptr(x), ptr(w.q), ptr(w.scale), ptr(out),
+             ptr(bias), ptr(resid), ll(x.stride(0)), ll(w.q.stride(0)), ll(w.scale.stride(0)), ll(out.stride(0)),
+             ll(resid.stride(0) if resid is not None else 0), c_int(m), c_int(N), c_int(K), c_int(epilogue),
+             c_int(1 if out.dtype == torch.float32 else 0), stream_ptr())
+        return out
     call("mm_skinny_gemm_wide" if wide else "mm_skinny_gemm", ptr(x), ptr(w), ptr(out), ptr(bias), ptr(resid), ll(x.stride(0)),
          ll(w.stride(0)), ll(out.stride(0)), ll(resid.stride(0) if resid is not None else 0), c_int(m),
          c_int(N), c_int(K), c_int(epilogue), c_int(1 if out.dtype == torch.float32 else 0), stream_ptr())
